@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""Benchmark of the Prompt-Free-Diffusion hot path on B200 (contract: see the task statement).
+"""Benchmark of the Prompt-Free-Diffusion hot path on an H100.
 
-  python bench.py --gpus N --steps K --warmup W [--config C]   # our CUDA path (pfd_b200)
+  python bench.py --gpus N --steps K --warmup W [--config C] [--dump-outputs DIR]   # our CUDA path (pfd_b200)
   python bench.py --impl reference --gpus N --steps K ...      # the reference's own CPU path on the host cores
-                                                               # (unmodified reference modules from baseline/_ref;
+                                                               # (unmodified reference modules from oracle/_ref;
                                                                #  oracle port when the staged copy is absent)
 
 Workloads = BASELINE.json configs (SURVEY.md §8d), per GPU; --config 2 (the one the metric is quoted on) is the
@@ -62,6 +62,8 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-gpu-reference", action="store_true")
     ap.add_argument("--no-graph", action="store_true")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the images of the last timed step to DIR/<name>.npy (float32) for output comparisons")
     a = ap.parse_args()
     cfg = dict(CONFIGS[a.config])
     if a.batch:
@@ -186,7 +188,7 @@ class quiet:
 
 # ------------------------------------------------------------------------------------------------ reference arms
 def build_reference(cfg):
-    """The UNMODIFIED reference pipeline (tools/ref_harness.py -> baseline/_ref or /root/reference) on the CPU with the
+    """The UNMODIFIED reference pipeline (tools/ref_harness.py -> oracle/_ref) on the CPU with the
     same synthetic weights (random init skipped: every tensor is overwritten).  Returns (net, RefSampler class) or None."""
     import torch
     import ref_harness as rh
@@ -217,7 +219,7 @@ def reference_gpu_leg(cfg, steps=2, warmup=1, gpu_index=0):
     import torch
     built = build_reference(cfg)
     if built is None:
-        return {"unavailable": "reference tree not staged (baseline/_ref missing)"}
+        return {"unavailable": "reference tree not staged (oracle/_ref missing)"}
     net, RefSampler = built
     net = net.half()
     net.to("cuda")
@@ -258,7 +260,7 @@ def reference_gpu_leg(cfg, steps=2, warmup=1, gpu_index=0):
     clk = clocks.stop()
     res = {"value": B * steps / (ms / 1000.0), "unit": "images/s", "ms_per_request": ms / steps, "requests": steps,
            "warmup": warmup,
-           "impl": "unmodified reference modules (baseline/_ref), torch %s eager fp16, no xformers" % torch.__version__,
+           "impl": "unmodified reference modules (oracle/_ref), torch %s eager fp16, no xformers" % torch.__version__,
            "peak_mem_gb": torch.cuda.max_memory_allocated() / 2 ** 30, "clocks": clk,
            "output_finite": bool(torch.isfinite(im.float()).all().item())}
     del net, sampler
@@ -350,7 +352,7 @@ def run_reference_gpu(args):
 
 # ------------------------------------------------------------------------------------------------
 def gemm_roofline_pass(net, cfg, cond, uncond, hint):
-    """Device time of the dominant kernel (pfd_gemm_f16 = tcgen05 GEMM / implicit-GEMM conv) inside ONE
+    """Device time of the dominant kernel (pfd_gemm_f16 = wgmma GEMM / implicit-GEMM conv) inside ONE
     CFG-pair UNet(+ControlNet) evaluation, measured live with CUDA events and without host-launch gaps: the
     evaluation is captured into a CUDA graph twice - once complete, once with every pfd_gemm_f16 launch elided - and
     both graphs are replayed back to back; kernel time = T_full - T_without.
@@ -435,15 +437,6 @@ def gemm_roofline_pass(net, cfg, cond, uncond, hint):
     return stats["flops"], max(t_full - t_nogemm, 1e-6), stats["n"], br
 
 
-def load_traffic():
-    """DRAM traffic of the dominant kernel from the committed ncu --set full capture (profiles/r2_traffic.json:
-    dram__bytes_read.sum + dram__bytes_write.sum per launch of the named shape, algorithmic bytes beside it)."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "r2_traffic.json")))
-    except Exception:
-        return None
-
-
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -456,11 +449,6 @@ def run_ours(args):
     from pfd_b200 import DDIMSampler, native as nv, parallel as par
     nv.load()
     cfg = args.cfg
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
     net = synth_net(cfg).half()
     net.to("cuda")
     if cfg["pa"]:
@@ -516,6 +504,8 @@ def run_ours(args):
         im, cond, uncond = request(img_dev)
     e1.record()
     sync_all()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"images": im})
     launches = nv.launch_count() - n0
     ms = e0.elapsed_time(e1)
     clk = clocks.stop()
@@ -564,20 +554,18 @@ def run_ours(args):
         stage_ms = {"seecoder_encode": t_ctx, "ddim_sampling": t_smp, "vae_decode": t_vae}
 
     if rank == 0:
-        peak_t = peaks.get("bf16_tflops_sustained", 1400.0)
-        which = "of measured (sustained, MEASURED_PEAKS.json)" if peaks else "of fallback"
+        peak_t = 989.0
+        which = "H100 SXM data sheet, dense fp16 tensor (700 W card; not a measured rate)"
         roofline = None
         if not split:
             flops, gms, nl, breakdown = gemm_roofline_pass(net, cfg, cond[:B], uncond[:B], hint)
             achieved = flops / (gms / 1000.0) / 1e12 if gms > 0 else 0.0
-            traffic = load_traffic()
             evals = len(range(0, 1000, 1000 // cfg["ddim_steps"]))
             if stage_ms is not None:
                 breakdown["sampler_overhead_ms"] = stage_ms["ddim_sampling"] - evals * breakdown["unet_eval_ms"]
-            roofline = {"bound": "tensor", "kernel": "pfd::gemm_tc_kernel<BN> (tcgen05 GEMM / implicit-GEMM conv)",
+            roofline = {"bound": "tensor", "kernel": "pfd::gemm_wgmma_kernel<BN> (wgmma GEMM / implicit-GEMM conv)",
                         "achieved": achieved, "peak": peak_t, "unit": "TFLOP/s", "frac": achieved / peak_t,
-                        "traffic": None if traffic is None else traffic.get("dram_bytes_per_launch"),
-                        "traffic_detail": traffic, "peak_source": which, "launches_in_unet_eval": nl,
+                        "peak_source": which, "launches_in_unet_eval": nl,
                         "algorithmic_gflop_in_unet_eval": flops / 1e9, "kernel_ms_in_unet_eval": gms,
                         "how": "CUDA events around graph replays of one CFG-pair UNet eval, with minus without the kernel's launches",
                         "unet_eval_breakdown_ms": breakdown,
@@ -610,7 +598,7 @@ def run_ours(args):
                            "parallelism": (f"dp{world}: ONE request of {B} images sharded (parallel.py: rank-0 encode + broadcast, "
                                            "full-batch randn + slice, all-gather of images)") if split else
                                           f"dp{world} (one request of {B} images per GPU, no data-path collective)",
-                           "l2": "working set (1.7 GB weights + GBs of activations per step) is larger than the 126 MB L2",
+                           "l2": "working set (1.7 GB weights + GBs of activations per step) is larger than the 50 MB L2",
                            "cuda_graph": False if args.no_graph else f"all {cfg['ddim_steps']} DDIM steps in one captured graph"},
                 "roofline": roofline, "cpu_baseline": cpu_baseline, "gpu_reference": gpu_ref,
                 "e2e": {"value": e2e, "unit": "images/s", "h2d_bytes_per_step": img_host.numel() * 2,
@@ -619,6 +607,26 @@ def run_ours(args):
         print(json.dumps(line), flush=True)
     if world > 1:
         dist.destroy_process_group()
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(dirname, arrays):
+    """Each array -> DIR/<name>.npy as float32.  An array above the size limit is replaced by a fixed, seeded sample of
+    its flattened elements (<name>_sample.npy) with their flat indices (<name>_sample_index.npy, float64)."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    per = DUMP_LIMIT_BYTES // max(1, len(arrays))
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if a.nbytes <= per:
+            np.save(os.path.join(dirname, f"{name}.npy"), a)
+            continue
+        n = per // 12                                                     # 4 B value + 8 B index per element
+        idx = np.sort(np.random.default_rng(0).choice(a.size, size=n, replace=False))
+        np.save(os.path.join(dirname, f"{name}_sample.npy"), a.reshape(-1)[idx])
+        np.save(os.path.join(dirname, f"{name}_sample_index.npy"), idx.astype(np.float64))
 
 
 def main():

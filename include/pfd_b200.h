@@ -1,5 +1,5 @@
 /*
- * pfd_b200 — C ABI of the B200 (sm_100a) kernel library behind the Prompt-Free-Diffusion hot path.
+ * pfd_b200 — C ABI of the H100 (sm_90a) kernel library behind the Prompt-Free-Diffusion hot path.
  *
  * The reference (SHI-Labs/Prompt-Free-Diffusion) has NO native boundary: every op on the path is a
  * torch/ATen library call made from lib/model_zoo/*.py.  This header is therefore the boundary a
@@ -47,15 +47,13 @@ PFD_API const char* pfd_last_error(void);
 PFD_API int64_t pfd_launch_count(void);
 /* Run-time tuning switches, so that variants can be A/B-timed inside one process (tools/ab_unet.py); name == NULL
  * resets all of them to the built-in defaults.  Unknown names are stored and ignored.  Known names (default):
- *   gemm_tma_epi (1)   TMA-store epilogue of pfd_gemm_f16 for plain channel-last outputs (0 = register epilogue)
- *   gemm_pair (0)      1 = CTA-pair kernel (cta_group::2) for long-K contractions, 2 = wherever applicable
  *   gemm_streamk (0)   stream-K tail of the persistent GEMM
- *   xattn_short (1)    persistent single-score-tile kernel of pfd_flash_attn_* for Nk <= 160, d <= 48
- *   flash_poly_mod (0) exponent path of the attention softmax: 1 = packed-half MUFU, n > 1 = every n-th pair on the FMA pipe */
+ *   flash_poly_mod (0) exponent path of the attention softmax for d <= 64: 1 = packed-half MUFU, n > 1 = every n-th
+ *                      pair on the FMA pipe */
 PFD_API int pfd_set_option(const char* name, int32_t value);
 
 /*
- * pfd_gemm_f16 — the tcgen05 tensor-core contraction used for every Linear, 1x1 conv, 3x3 conv
+ * pfd_gemm_f16 — the wgmma tensor-core contraction used for every Linear, 1x1 conv, 3x3 conv
  * (implicit GEMM, TMA does the im2col) and batched QK^T / PV product on the path.
  *
  *   out[n, y, x, :] = act( alpha * sum_seg sum_tap sum_c A_seg[n, y*s+dy-1+o, x*s+dx-1+o, c] * Wt[:, k(seg,tap,c)]
@@ -209,7 +207,7 @@ PFD_API int pfd_patch_merge_gather_f16(const void* x, int32_t B, int32_t H, int3
                                void* out, void* stream);
 
 /*
- * Fused flash attention (tcgen05): out[b, i, h*d + :] = softmax_j( fp16(q_i . k_j) * scale ) @ v  per (b, h),
+ * Fused flash attention (wgmma): out[b, i, h*d + :] = softmax_j( fp16(q_i . k_j) * scale ) @ v  per (b, h),
  * scores never leave the SM.  Replaces attention.py:186-201 (einsum -> softmax -> einsum) for the UNet /
  * ControlNet self- and cross-attention.
  *   q  [B*heads, q_rows, d]   (first Nq rows valid)      k [B*heads, k_rows, d] (first Nk rows valid)

@@ -1,4 +1,4 @@
-"""pfd_b200 — B200-native (sm_100a) implementation of the Prompt-Free-Diffusion inference hot path.
+"""pfd_b200 — H100-native (sm_90a) implementation of the Prompt-Free-Diffusion inference hot path.
 
 Public surface (mirrors the reference's lib.model_zoo / lib.cfg_helper plugin API):
     from pfd_b200 import get_model, register, model_cfg_bank, DDIMSampler

@@ -19,7 +19,7 @@ import torch
 from . import native as nv
 
 
-# fused tcgen05 flash attention for bias-free attention; False falls back to the materialised
+# fused wgmma flash attention for bias-free attention; False falls back to the materialised
 # QK^T GEMM -> softmax -> PV GEMM pipeline (still all pfd_b200 kernels) — used by tests to cross-check.
 USE_FLASH = True
 # fused q|k projection + V^T produced by a "swapped" GEMM (Wv . X^T), consumed by the v1 kernel through strided views

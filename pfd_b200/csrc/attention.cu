@@ -1,24 +1,18 @@
-// Attention kernels for sm_100a (tcgen05 + TMEM + TMA) of the UNet / ControlNet / SeeCoder self- and cross-attention
+// Fused attention for sm_90a (wgmma + TMA + mbarrier) of the UNet / ControlNet / SeeCoder self- and cross-attention
 // (attention.py:178-201):  O = softmax(Q K^T * scale) V  per (batch, head), the [N, Nk] score matrix never reaches HBM.
 //
 // flash_attn_kernel (any Nk, d <= 192):
-//   CTA = 128 query rows of one (batch, head); KV processed in blocks of 64 keys.
-//   warp 0      : TMA producer (Q once; K through a 2-stage ring, V^T through a 1- or 2-stage ring)
-//   warp 1      : tcgen05.mma issuer   S_j = Q K_j^T  (TMEM)   O += P_j V_j (TMEM)
-//   warps 2..5  : softmax: thread r owns query row r (TMEM lane r) -> no cross-thread reductions; ONE pass over S_j:
-//                 tcgen05.ld of the 64 fp32 logits -> 3-input max chains -> p = ex2(s * scale * log2e - m) in fp32 ->
-//                 fp16 P written to shared memory in the K-major 128B-swizzled layout the PV MMA reads.  The running
-//                 reference exponent m only moves when a block maximum exceeds it by more than 2^8 (lazy rescaling),
-//                 so the TMEM read-modify-write of O is rare; final O / l written as [B, Nq, heads*d].
-//   The row sum l comes for free from the tensor core: row d of the V^T tile is all ones, so column d of the O
-//   accumulator is sum_j p_j of the fp16-rounded probabilities (numerator and denominator stay consistent).
-//   d <= 64: 55 KB of shared memory, 128 TMEM columns, 80 registers -> four CTAs per SM overlap each other's
-//   TMEM-load / MUFU / barrier phases (the kernel is bound by the XU pipe and by the length of the
-//   S -> softmax -> P -> PV hand-off chain, not by the tensor pipe: 4 * d = 160 MMA flops per exponential).
-//   Optional exponent paths for A/B (flash_poly_mod): packed-half MUFU (1), polynomial on the FMA pipe for every n-th pair.
-//
-// xattn_short_kernel (Nk <= 160, d <= 48): persistent single-score-tile kernel for the cross-attention against the 148
-//   context tokens, see below.
+//   CTA = 128 query rows of one (batch, head); keys processed in blocks of 64.
+//   warps 0..7 : two consumer warpgroups, 64 query rows each:
+//                S_j = Q K_j^T        wgmma, A = Q and B = K_j from shared memory, fp32 logits in registers;
+//                online softmax       row max / sum over the 4 threads of a row (2 shuffles), p = 2^(s*scale*log2e - m)
+//                                     rounded to fp16, the running output rescaled in registers when m moves;
+//                O += P_j V_j         wgmma with A = P straight from registers (the S accumulator fragment is the A
+//                                     operand fragment), B = the V^T block (d rows x 64 keys, K-major) from shared memory.
+//   warp 8     : TMA producer (Q once; K and V^T blocks through 2-stage rings released by the consumer warps).
+//   The row sum l accumulates the fp16-rounded probabilities, the values the PV product actually uses.
+//   Optional exponent paths (flash_poly_mod, d <= 64): packed-half MUFU (1), polynomial on the FMA pipe for every
+//   n-th pair (n > 1).
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -28,19 +22,16 @@
 #include "../../include/pfd_b200.h"
 #include "common.h"
 #include "ptx.cuh"
+#include "wgmma.cuh"
 
 namespace pfd {
 
 constexpr int FA_BQ = 128;
 constexpr int FA_BKV = 64;
-constexpr int FA_THREADS = 192;
+constexpr int FA_THREADS = 288;       // 2 consumer warpgroups + 1 producer warp
 constexpr int FLASH_POLY_MOD_DEFAULT = 0;
 
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-  float d;
-  asm("max.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
-  return d;
-}
+__device__ __forceinline__ float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
 __device__ __forceinline__ uint32_t ex2_f16x2(uint32_t x) {
   uint32_t y;
   asm("ex2.approx.f16x2 %0, %1;" : "=r"(y) : "r"(x));
@@ -83,61 +74,54 @@ struct alignas(64) FlashParams {
   long long o_sb, o_sq, o_sh;  // element strides: batch, query row, head
 };
 
-template <int DCH>
+// DCH: 64-wide chunks of the head dim (Q / K tiles); DP: head dim padded to the wgmma N granule of 16 (V^T rows)
+template <int DCH, int DP>
 struct FlashCfg {
   static constexpr int Q_BYTES = DCH * FA_BQ * 128;
   static constexpr int K_BYTES = DCH * FA_BKV * 128;
-  static constexpr int DN = DCH == 1 ? 80 : (DCH == 2 ? 144 : 208);  // max rows of the V^T tile (d + ones row, padded)
-  static constexpr int P_BYTES = FA_BQ * 128;
-  static constexpr int NPB = 1;                  // P buffers
-  // S accumulators in TMEM: one for d <= 64 (64 + 48 columns -> 128-column allocation, ~60 KB smem ->
-  // three CTAs per SM overlap each other's TMEM-load / MUFU / smem / MMA phases), two otherwise
-  static constexpr int NSB = DCH == 1 ? 1 : 2;
-  // K/V smem stages
-  //
-  static constexpr int NKV = 2;   // K stages (1 stage was measured 55% slower: the QK^T of block j+1 must overlap softmax j)
-  // V^T stages: V_j is only needed by PV_j, a full softmax after K_j, so for d <= 64 one stage is enough and the
-  // CTA fits four to an SM (55 KB, 128 TMEM columns, <= 85 registers): 16 softmax warps hide each other's
-  // TMEM-load / MUFU / barrier phases better than 12
-  static constexpr int NVS = DCH == 1 ? 1 : 2;
-  static constexpr int MIN_CTAS = DCH == 1 ? 4 : 2;
-  // V^T stage = dN rows x 128 B (dN = ceil16(d + 1), runtime) so d=80 still fits two CTAs per SM
-  static int smem_bytes(int dN) { return Q_BYTES + NKV * K_BYTES + NVS * dN * 128 + NPB * P_BYTES + 1024 + 128; }
+  static constexpr int V_BYTES = DP * 128;
+  static constexpr int SMEM_BYTES = Q_BYTES + 2 * K_BYTES + 2 * V_BYTES + 1024 + 128;
+  static_assert(DP % 16 == 0 && DP <= 64 * DCH, "V^T rows");
 };
+
+__device__ __forceinline__ uint32_t pack_f2h(float a, float b) {
+  const __half2 h = __floats2half2_rn(a, b);
+  return *reinterpret_cast<const uint32_t*>(&h);
+}
 
 // PM > 1: every PM-th pair of exponentials of a key block takes the polynomial path (exp2_poly_h2) instead of MUFU;
 // PM = 1: every pair goes through ONE packed-half MUFU op (ex2.approx.f16x2)
-template <int DCH, int PM>
-__global__ void __launch_bounds__(FA_THREADS, FlashCfg<DCH>::MIN_CTAS)
+template <int PM>
+__device__ __forceinline__ uint32_t exp2_pair(float t0, float t1, int pair) {
+  if (PM == 1) {
+    // both exponentials in ONE MUFU op on packed halves (t <= 0 rounded to fp16 first: the exponent error is <= 2^-7 for
+    // the smallest terms and <= 2^-11 for the ones that matter - the size of the fp16 rounding of the reference's own
+    // score tensor, attention.py:188)
+    const __half2 th = __floats2half2_rn(t0, t1);
+    return ex2_f16x2(*reinterpret_cast<const uint32_t*>(&th));
+  }
+  if (PM > 1 && (pair % (PM > 1 ? PM : 2)) == (PM > 1 ? PM : 2) - 1) return exp2_poly_h2(t0, t1);
+  return pack_f2h(fast_exp2(t0), fast_exp2(t1));
+}
+
+template <int DCH, int DP, int PM>
+__global__ void __launch_bounds__(FA_THREADS, DCH == 1 ? 2 : 1)
 flash_attn_kernel(const __grid_constant__ FlashParams p) {
-  using Cfg = FlashCfg<DCH>;
+  using Cfg = FlashCfg<DCH, DP>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_addr = smem_u32(smem_raw);
   const uint32_t base = (raw_addr + 1023u) & ~1023u;
   uint8_t* gbase = smem_raw + (base - raw_addr);
   const int d = p.d;
-  const int dN = (d + 16) & ~15;       // PV MMA N: d value rows + the all-ones row (-> row sums), padded to 16
-  const int V_BYTES = dN * 128;
-  const uint32_t need_cols = Cfg::NSB * FA_BKV + dN;
-  const uint32_t tmem_cols = need_cols <= 128 ? 128u : (need_cols <= 256 ? 256u : 512u);
   const uint32_t sQ = base;
   const uint32_t sK = sQ + Cfg::Q_BYTES;                  // [2][K_BYTES]
-  const uint32_t sV = sK + Cfg::NKV * Cfg::K_BYTES;       // [NVS][V_BYTES]
-  const uint32_t sP = sV + Cfg::NVS * V_BYTES;
-  const uint32_t bars = sP + Cfg::NPB * Cfg::P_BYTES;
-  uint8_t* gP = gbase + Cfg::Q_BYTES + Cfg::NKV * Cfg::K_BYTES + Cfg::NVS * V_BYTES;
+  const uint32_t sV = sK + 2 * Cfg::K_BYTES;              // [2][V_BYTES]
+  const uint32_t bars = sV + 2 * Cfg::V_BYTES;
   const uint32_t bar_q = bars;
-  auto bar_k_full = [&](int s) { return bars + 8u * (1 + s); };
-  auto bar_k_empty = [&](int s) { return bars + 8u * (3 + s); };
-  auto bar_v_full = [&](int s) { return bars + 8u * (12 + s); };
-  auto bar_v_empty = [&](int s) { return bars + 8u * (14 + s); };
-  auto bar_s_full = [&](int s) { return bars + 8u * (5 + s); };
-  auto bar_s_free = [&](int s) { return bars + 8u * (7 + s); };
-  const uint32_t bar_p_ready = bars + 8u * 9;
-  const uint32_t bar_pv_done = bars + 8u * 10;
-  const uint32_t tmem_slot = bars + 8u * 11;
-  volatile uint32_t* tmem_slot_g = reinterpret_cast<volatile uint32_t*>(
-      gbase + Cfg::Q_BYTES + Cfg::NKV * Cfg::K_BYTES + Cfg::NVS * V_BYTES + Cfg::NPB * Cfg::P_BYTES + 8 * 11);
+  auto k_full = [&](int s) { return bars + 8u * (1 + s); };
+  auto k_empty = [&](int s) { return bars + 8u * (3 + s); };
+  auto v_full = [&](int s) { return bars + 8u * (5 + s); };
+  auto v_empty = [&](int s) { return bars + 8u * (7 + s); };
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -146,560 +130,162 @@ flash_attn_kernel(const __grid_constant__ FlashParams p) {
   const int hb = bh % p.heads, bb = bh / p.heads;
   const int nblk = p.nblk;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 256) {
     tma_prefetch_desc(&p.tmQ);
     tma_prefetch_desc(&p.tmK);
     tma_prefetch_desc(&p.tmV);
-  }
-  if (warp == 1 && lane == 0) {
     mbar_init(bar_q, 1);
     for (int s = 0; s < 2; ++s) {
-      mbar_init(bar_k_full(s), 1);
-      mbar_init(bar_k_empty(s), 1);
-      mbar_init(bar_v_full(s), 1);
-      mbar_init(bar_v_empty(s), 1);
-      mbar_init(bar_s_full(s), 1);
-      mbar_init(bar_s_free(s), 128);
+      mbar_init(k_full(s), 1);
+      mbar_init(k_empty(s), 8);            // one arrival per consumer warp
+      mbar_init(v_full(s), 1);
+      mbar_init(v_empty(s), 8);
     }
-    mbar_init(bar_p_ready, 128);
-    mbar_init(bar_pv_done, 1);
     mbar_fence_init();
   }
-  if (warp == 2) tmem_alloc_rt(tmem_slot, tmem_cols);
-  if (warp >= 2) {
-    // rows d..dN-1 of the V^T stages are never written by TMA (its box has d rows): row d = ones, rest = 0
-    uint8_t* gV = gbase + Cfg::Q_BYTES + Cfg::NKV * Cfg::K_BYTES;
-    const int t = threadIdx.x - 64;
-    const int per_stage = (dN - d) * 8;               // 16-byte granules
-    for (int i = t; i < Cfg::NVS * per_stage; i += 128) {
+  if (DP > d && warp < 8) {
+    // rows d..DP-1 of the V^T stages are never written by TMA (its box has d rows): zero, so the padded output
+    // columns stay finite
+    const int per_stage = (DP - d) * 8;               // 16-byte granules
+    for (int i = threadIdx.x; i < 2 * per_stage; i += 256) {
       const int st = i / per_stage, g = i % per_stage;
-      const uint32_t word = (g < 8) ? 0x3C003C00u : 0u;
-      *reinterpret_cast<uint4*>(gV + st * V_BYTES + d * 128 + g * 16) = make_uint4(word, word, word, word);
+      *reinterpret_cast<uint4*>(gbase + Cfg::Q_BYTES + 2 * Cfg::K_BYTES + st * Cfg::V_BYTES + d * 128 + g * 16) =
+          make_uint4(0, 0, 0, 0);
     }
     fence_proxy_async_smem();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_g;
-  const uint32_t tmem_O = tmem_base + Cfg::NSB * FA_BKV;
   pdl_wait();                  // q / k / v are produced by the preceding projection GEMMs
   pdl_launch_dependents();
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       mbar_expect_tx(bar_q, Cfg::Q_BYTES);
       for (int c = 0; c < DCH; ++c) tma_load_4d(sQ + c * FA_BQ * 128, &p.tmQ, bar_q, c * 64, q0, hb, bb);
-      auto issue_K = [&](int j) {
-        const int st = j % Cfg::NKV, u = j / Cfg::NKV;
-        if (u >= 1) mbar_wait(bar_k_empty(st), (u - 1) & 1);          // QK^T of block j - NKV has read the stage
-        mbar_expect_tx(bar_k_full(st), Cfg::K_BYTES);
-        for (int c = 0; c < DCH; ++c)
-          tma_load_4d(sK + st * Cfg::K_BYTES + c * FA_BKV * 128, &p.tmK, bar_k_full(st), c * 64, j * FA_BKV, hb, bb);
-      };
-      auto issue_V = [&](int j) {
-        const int st = j % Cfg::NVS, u = j / Cfg::NVS;
-        if (u >= 1) mbar_wait(bar_v_empty(st), (u - 1) & 1);          // PV of block j - NVS has read the stage
-        mbar_expect_tx(bar_v_full(st), d * 128);
-        tma_load_4d(sV + st * V_BYTES, &p.tmV, bar_v_full(st), j * FA_BKV, 0, hb, bb);
-      };
-      // K runs one block ahead of V: K_{j+1} feeds the QK^T that overlaps softmax j, V_j is only needed by PV_j
-      issue_K(0);
-      issue_V(0);
-      if (nblk > 1) issue_K(1);
-      for (int j = 1; j < nblk; ++j) {
-        if (j + 1 < nblk) issue_K(j + 1);
-        issue_V(j);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc_s = make_idesc_f16(FA_BKV);
-      const uint32_t idesc_o = make_idesc_f16((uint32_t)dN);
-      auto issue_S = [&](int j) {
-        const int st = j % Cfg::NKV;
-        const int sb = j % Cfg::NSB;
-        const uint32_t tS = tmem_base + sb * FA_BKV;
-        bool first = true;
-        for (int c = 0; c < DCH; ++c) {
-          const int rem = d - c * 64;
-          if (rem <= 0) break;
-          const int ksteps = rem >= 64 ? 4 : (rem + 15) / 16;
-          const uint64_t ad = make_sw128_kmajor_desc(sQ + c * FA_BQ * 128);
-          const uint64_t bd = make_sw128_kmajor_desc(sK + st * Cfg::K_BYTES + c * FA_BKV * 128);
-          for (int s = 0; s < ksteps; ++s) {
-            umma_f16(tS, ad + 2u * s, bd + 2u * s, idesc_s, first ? 0u : 1u);
-            first = false;
-          }
-        }
-        umma_commit(bar_s_full(sb));
-        umma_commit(bar_k_empty(st));
-      };
-      mbar_wait(bar_q, 0);
-      mbar_wait(bar_k_full(0), 0);
-      tc_fence_after();
-      issue_S(0);
       for (int j = 0; j < nblk; ++j) {
-        auto next_S = [&]() {
-          if (j + 1 < nblk) {
-            const int st = (j + 1) % Cfg::NKV, u = (j + 1) / Cfg::NKV;
-            const int sb = (j + 1) % Cfg::NSB, us = (j + 1) / Cfg::NSB;
-            mbar_wait(bar_k_full(st), u & 1);
-            if (us >= 1) mbar_wait(bar_s_free(sb), (us - 1) & 1);
-            tc_fence_after();
-            issue_S(j + 1);
-          }
-        };
-        // QK^T of block j+1 is issued before PV of block j (overlaps the softmax of j)
-        next_S();
-        mbar_wait(bar_p_ready, j & 1);
-        const int st = j % Cfg::NVS;
-        mbar_wait(bar_v_full(st), (j / Cfg::NVS) & 1);
-        tc_fence_after();
-        const uint64_t ad = make_sw128_kmajor_desc(sP + (Cfg::NPB == 2 ? (j & 1) * Cfg::P_BYTES : 0));
-        const uint64_t bd = make_sw128_kmajor_desc(sV + st * V_BYTES);
-#pragma unroll
-        for (int s = 0; s < FA_BKV / 16; ++s)
-          umma_f16(tmem_O, ad + 2u * s, bd + 2u * s, idesc_o, (j > 0 || s > 0) ? 1u : 0u);
-        umma_commit(bar_v_empty(st));
-        umma_commit(bar_pv_done);
+        const int st = j & 1, u = j >> 1;
+        if (u >= 1) mbar_wait(k_empty(st), (u - 1) & 1);          // S of block j - 2 has read the stage
+        mbar_expect_tx(k_full(st), Cfg::K_BYTES);
+        for (int c = 0; c < DCH; ++c)
+          tma_load_4d(sK + st * Cfg::K_BYTES + c * FA_BKV * 128, &p.tmK, k_full(st), c * 64, j * FA_BKV, hb, bb);
+        if (u >= 1) mbar_wait(v_empty(st), (u - 1) & 1);          // PV of block j - 2 has read the stage
+        mbar_expect_tx(v_full(st), d * 128);
+        tma_load_4d(sV + st * Cfg::V_BYTES, &p.tmV, v_full(st), j * FA_BKV, 0, hb, bb);
       }
     }
-  } else {
-    // ------------------------------------------------------------------ softmax / output warps
-    const int qd = warp & 3;
-    const int row = qd * 32 + lane;
-    const uint32_t lane_off = static_cast<uint32_t>(qd * 32) << 16;
-    const float LOG2E = 1.4426950408889634f;
-    const float c2 = p.scale * LOG2E;                   // logits in log2 units: t = s * c2
-    // Running reference exponent (log2 units).  It only moves when the block maximum exceeds it by more than
-    // RESCALE_TAU (lazy rescaling: P <= 2^TAU stays far inside fp16 range and the fp32 accumulators absorb the
-    // common factor, which cancels in O / l), so the TMEM read-modify-write of O is rare after the first blocks.
-    constexpr float RESCALE_TAU = 8.f;
-    float mref = -INFINITY;
-    uint8_t* prow0 = gP + row * 128;
-    const int rsw = row & 7;
-    for (int j = 0; j < nblk; ++j) {
-      const int sb = j % Cfg::NSB, us = j / Cfg::NSB;
-      const int kvalid = min(FA_BKV, p.Nk - j * FA_BKV);
-      const bool partial = kvalid < FA_BKV;            // block-uniform
-      mbar_wait(bar_s_full(sb), us & 1);
-      tc_fence_after();
-      const uint32_t tS = tmem_base + lane_off + sb * FA_BKV;
-      // single pass over S (fp32 logits of this thread's query row against 64 keys)
-      uint32_t r[FA_BKV];
-      tmem_ld32(tS, *reinterpret_cast<uint32_t(*)[32]>(&r[0]));
-      tmem_ld32(tS + 32, *reinterpret_cast<uint32_t(*)[32]>(&r[32]));
-      tmem_ld_wait();
-      tc_fence_before();
-      mbar_arrive(bar_s_free(sb));                      // S buffer may now be overwritten by the next QK^T
-      if (partial) {
+    return;
+  }
+
+  // ------------------------------------------------------------------ consumer warpgroups
+  const int cw = warp >> 2;                  // rows [64 cw, 64 cw + 64) of the query tile
+  const int wl = warp & 3;
+  const int tq = lane & 3;
+  const float c2 = p.scale * 1.4426950408889634f;   // logits in log2 units: t = s * c2
+  float o[DP / 2];
 #pragma unroll
-        for (int i = 0; i < FA_BKV; ++i)
-          if (i >= kvalid) r[i] = 0xff800000u;          // -inf: masked keys contribute exp2(-inf) = 0
-      }
-      // block maximum: four independent 3-input max chains
-      float mx[4];
+  for (int i = 0; i < DP / 2; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  mbar_wait(bar_q, 0);
+  for (int j = 0; j < nblk; ++j) {
+    const int st = j & 1;
+    const uint32_t ph = (j >> 1) & 1;
+    mbar_wait(k_full(st), ph);
+    float s[FA_BKV / 2];
 #pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        mx[q] = fmax3(__uint_as_float(r[q * 16]), __uint_as_float(r[q * 16 + 1]), __uint_as_float(r[q * 16 + 2]));
+    for (int i = 0; i < FA_BKV / 2; ++i) s[i] = 0.f;
+    wgmma_fence();
 #pragma unroll
-        for (int i = 3; i + 1 < 16; i += 2)
-          mx[q] = fmax3(mx[q], __uint_as_float(r[q * 16 + i]), __uint_as_float(r[q * 16 + i + 1]));
-        mx[q] = fmaxf(mx[q], __uint_as_float(r[q * 16 + 15]));
-      }
-      const float mb = fmax3(fmaxf(mx[0], mx[1]), mx[2], mx[3]) * c2;
-      const bool move = mb > mref + RESCALE_TAU;        // always true for j == 0 (mref = -inf)
-      const float mnew = move ? mb : mref;
-      const float alpha = move ? fast_exp2(mref - mnew) : 1.f;   // j == 0: exp2(-inf) = 0, unused
-      mref = mnew;
-      const float nm = -mnew;
-      // p = 2^(s * c2 - mref) -> packed fp16 (registers), overlapping PV_{j-1}
-      uint32_t pk[FA_BKV / 2];
+    for (int c = 0; c < DCH; ++c) {
+      const uint64_t ad = make_sw128_kmajor_desc(sQ + c * FA_BQ * 128 + cw * 64 * 128);
+      const uint64_t bd = make_sw128_kmajor_desc(sK + st * Cfg::K_BYTES + c * FA_BKV * 128);
 #pragma unroll
-      for (int i = 0; i < FA_BKV / 2; ++i) {
-        const float t0 = fmaf(__uint_as_float(r[2 * i]), c2, nm);
-        const float t1 = fmaf(__uint_as_float(r[2 * i + 1]), c2, nm);
-        if (PM == 1) {
-          // both exponentials of the pair in ONE MUFU op on packed halves (t rounded to fp16 first: |t| <= 16, so the
-          // exponent error is <= 2^-7 for the smallest terms and <= 2^-11 for the ones that matter - the size of the fp16
-          // rounding of the reference's own score tensor, attention.py:188)
-          const __half2 th = __floats2half2_rn(t0, t1);
-          pk[i] = ex2_f16x2(*reinterpret_cast<const uint32_t*>(&th));
-        } else if (PM > 1 && (i % (PM > 1 ? PM : 2)) == (PM > 1 ? PM : 2) - 1) {
-          pk[i] = exp2_poly_h2(t0, t1);
-        } else {
-          const __half2 h = __floats2half2_rn(fast_exp2(t0), fast_exp2(t1));
-          pk[i] = *reinterpret_cast<const uint32_t*>(&h);
-        }
-      }
-      if (j > 0) {
-        // single P buffer / running O: PV_{j-1} must have consumed P and finished accumulating
-        mbar_wait(bar_pv_done, (j - 1) & 1);
-        tc_fence_after();
-      }
-      uint8_t* prow = prow0 + (Cfg::NPB == 2 ? (j & 1) * Cfg::P_BYTES : 0);
-#pragma unroll
-      for (int g = 0; g < FA_BKV / 8; ++g)
-        *reinterpret_cast<uint4*>(prow + ((g ^ rsw) << 4)) = make_uint4(pk[4 * g], pk[4 * g + 1], pk[4 * g + 2], pk[4 * g + 3]);
-      // rescale the running output (and its row-sum column) when a reference exponent of this warp moved
-      if (j > 0) {
-        const bool need = __any_sync(0xffffffffu, move);
-        if (need) {
-          for (int c = 0; c < dN / 16; ++c) {
-            uint32_t o[16];
-            tmem_ld16(tmem_O + lane_off + c * 16, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st16(tmem_O + lane_off + c * 16, o);
-          }
-          tmem_st_wait();
-        }
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(bar_p_ready);
+      for (int k = 0; k < 4; ++k)
+        if (c * 64 + k * 16 < d) Wgmma<FA_BKV>::ss(s, ad + 2u * k, bd + 2u * k, (c | k) != 0 ? 1u : 0u);
     }
-    // ---- epilogue: O / l -> [B, Nq, heads*d]   (l = column d of the accumulator)
-    mbar_wait(bar_pv_done, (nblk - 1) & 1);
-    tc_fence_after();
-    const uint32_t lraw = tmem_ld1(tmem_O + lane_off + d);
-    tmem_ld_wait();
-    const float l = __uint_as_float(lraw);
-    const int q = q0 + row;
-    const float inv = l > 0.f ? 1.f / l : 0.f;
-    const int b = bh / p.heads, h = bh % p.heads;
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (lane == 0) mbar_arrive(k_empty(st));
+    // mask keys beyond Nk (their K rows are TMA zero fill): column 8 jj + 2 tq + e of the block
+    const int kvalid = p.Nk - j * FA_BKV;
+    if (kvalid < FA_BKV) {
+#pragma unroll
+      for (int jj = 0; jj < FA_BKV / 8; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (8 * jj + 2 * tq + e >= kvalid) {
+            s[4 * jj + e] = -INFINITY;
+            s[4 * jj + 2 + e] = -INFINITY;
+          }
+    }
+    // row maxima (rows r0 = 16 wl + lane / 4 and r0 + 8): 16 values per thread, then across the 4 threads of the row
+    float mx[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      float a = fmax3(s[2 * i], s[2 * i + 1], s[4 + 2 * i]);
+      float b = fmax3(s[4 + 2 * i + 1], s[8 + 2 * i], s[8 + 2 * i + 1]);
+#pragma unroll
+      for (int jj = 3; jj < FA_BKV / 8; ++jj) {
+        if (jj & 1) b = fmax3(b, s[4 * jj + 2 * i], s[4 * jj + 2 * i + 1]);
+        else a = fmax3(a, s[4 * jj + 2 * i], s[4 * jj + 2 * i + 1]);
+      }
+      mx[i] = fmaxf(a, b);
+      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
+      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
+    }
+    float nm[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const float mnew = fmaxf(m[i], mx[i] * c2);
+      const float alpha = fast_exp2(m[i] - mnew);       // j == 0: exp2(-inf) = 0 (o and l are still 0)
+      m[i] = mnew;
+      nm[i] = -mnew;
+      l[i] *= alpha;
+#pragma unroll
+      for (int jj = 0; jj < DP / 8; ++jj) {
+        o[4 * jj + 2 * i] *= alpha;
+        o[4 * jj + 2 * i + 1] *= alpha;
+      }
+    }
+    // P = 2^(s c2 - m) in fp16, laid out as the A fragments of the four k16 steps of the PV product
+    uint32_t pa[4][4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const int i = r & 1;                    // row r0 (i = 0) or r0 + 8
+        const int idx = 8 * k + 4 * (r >> 1) + 2 * i;
+        const uint32_t h = exp2_pair<PM>(fmaf(s[idx], c2, nm[i]), fmaf(s[idx + 1], c2, nm[i]), 4 * k + r);
+        const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&h));
+        l[i] += hf.x + hf.y;
+        pa[k][r] = h;
+      }
+    }
+    mbar_wait(v_full(st), ph);
+    wgmma_fence();
+    const uint64_t vd = make_sw128_kmajor_desc(sV + st * Cfg::V_BYTES);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) Wgmma<DP>::rs(o, pa[k], vd + 2u * k, 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    if (lane == 0) mbar_arrive(v_empty(st));
+  }
+  // ---- epilogue: O / l -> [B, Nq, heads*d]
+  const int b = bh / p.heads, h = bh % p.heads;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float li = l[i];
+    li += __shfl_xor_sync(0xffffffffu, li, 1);
+    li += __shfl_xor_sync(0xffffffffu, li, 2);
+    const float inv = li > 0.f ? 1.f / li : 0.f;
+    const int q = q0 + cw * 64 + wl * 16 + (lane >> 2) + 8 * i;
+    if (q >= p.Nq) continue;
     __half* orow = p.out + (long long)b * p.o_sb + (long long)q * p.o_sq + (long long)h * p.o_sh;
-    for (int c = 0; c < (d + 15) / 16; ++c) {
-      uint32_t o[16];
-      tmem_ld16(tmem_O + lane_off + c * 16, o);
-      tmem_ld_wait();
-      if (q < p.Nq) {
 #pragma unroll
-        for (int h8 = 0; h8 < 2; ++h8) {
-          const int col = c * 16 + h8 * 8;
-          if (col < d) {
-            uint4 v;
-            __half2* hv = reinterpret_cast<__half2*>(&v);
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-              hv[i] = __floats2half2_rn(__uint_as_float(o[h8 * 8 + 2 * i]) * inv,
-                                        __uint_as_float(o[h8 * 8 + 2 * i + 1]) * inv);
-            *reinterpret_cast<uint4*>(orow + col) = v;
-          }
-        }
-      }
+    for (int jj = 0; jj < DP / 8; ++jj) {
+      const int col = 8 * jj + 2 * tq;
+      if (col < d)
+        *reinterpret_cast<__half2*>(orow + col) = __floats2half2_rn(o[4 * jj + 2 * i] * inv, o[4 * jj + 2 * i + 1] * inv);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_rt(tmem_base, tmem_cols);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------------------
-// Short-key attention: the UNet / ControlNet CROSS-attention against the 148 SeeCoder context tokens
-// (attention.py:178-201 with `context`; Nk = 148 at every level, d = 40 at the 64x64 level where 94 % of its
-// exponentials are).  All keys fit ONE score tile, so there is no online softmax: S = Q K^T is a single
-// 128 x 160 tcgen05.mma tile, the row maximum is exact, P is written once and O = P V^T is 10 k-steps.
-// The generic kernel above spends most of such a launch in per-CTA set-up (TMEM allocation, barrier init, cold Q
-// load: 3 key blocks per CTA, the third one 69 % padding); this one is PERSISTENT: each CTA walks a contiguous
-// range of (batch*head, query tile) items, K / V^T of a head stay in shared memory until the head changes, and
-// two softmax groups (8 warps each, two threads per query row) alternate items on private S / O accumulators and P
-// buffers so one group's MUFU phase
-// overlaps the other's TMEM loads, shared-memory stores and output epilogue.
-//   warp 0      : TMA producer (Q tile per item through a 2-slot ring; K + V^T per head through a 2-slot ring)
-//   warp 1      : tcgen05.mma issuer: S(0) S(1) [PV(i) S(i+2)]...
-//   warps 2..9  : softmax / epilogue group 0 (even items), warps 10..17: group 1 (odd items); warps wi and wi + 4
-//                 of a group share the query rows of a TMEM lane quarter and split the score columns 80 / 80
-// Barrier protocol (single arrival unless noted): q_full/q_empty[2], kv_full/kv_empty[2], s_full[2],
-// p_ready[2] (256 arrivals), o_full[2].  There is no s_free / o_free barrier: group g arrives on p_ready only
-// after it has read S_g completely and (one item earlier) drained O_g, and the issuer orders S(i+2) and PV(i+2)
-// behind the wait on p_ready(i) / p_ready(i+2).
-constexpr int XS_NKP = 160;        // score tile width (keys, padded to the UMMA N granule of 16)
-constexpr int XS_THREADS = 64 + 2 * 256;   // TMA warp, MMA warp, 2 softmax groups of 8 warps
-constexpr int XS_Q_BYTES = FA_BQ * 128;
-constexpr int XS_K_BYTES = XS_NKP * 128;
-constexpr int XS_P_BYTES = 3 * FA_BQ * 128;      // 3 chunks of 64 keys (the third one half used)
-
-struct alignas(64) XsParams {
-  CUtensorMap tmQ, tmK, tmV;
-  int Nq, Nk, heads, d;
-  int nqt, total;                  // query tiles per (batch, head); work items = B * heads * nqt
-  float scale;
-  __half* out;
-  long long o_sb, o_sq, o_sh;
-};
-
-static int xs_smem_bytes(int dN) { return 2 * XS_Q_BYTES + 2 * XS_K_BYTES + 2 * 3 * dN * 128 + 2 * XS_P_BYTES + 1024 + 256 + 2048; }
-
-template <int PM>
-__global__ void __launch_bounds__(XS_THREADS, 1)
-xattn_short_kernel(const __grid_constant__ XsParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw_addr = smem_u32(smem_raw);
-  const uint32_t base = (raw_addr + 1023u) & ~1023u;
-  uint8_t* gbase = smem_raw + (base - raw_addr);
-  const int d = p.d;
-  const int dN = (d + 16) & ~15;                 // value rows + the all-ones row (row sums), padded to 16
-  const int VC_BYTES = dN * 128;                 // one 64-key chunk of V^T
-  const int V_BYTES = 3 * VC_BYTES;
-  const uint32_t sQ = base;                      // [2][XS_Q_BYTES]
-  const uint32_t sK = sQ + 2 * XS_Q_BYTES;       // [2][XS_K_BYTES]
-  const uint32_t sV = sK + 2 * XS_K_BYTES;       // [2][3][VC_BYTES]
-  const uint32_t sP = sV + 2 * V_BYTES;          // [2][XS_P_BYTES]
-  const uint32_t bars = sP + 2 * XS_P_BYTES;
-  const int off_V = 2 * XS_Q_BYTES + 2 * XS_K_BYTES;
-  const int off_P = off_V + 2 * V_BYTES;
-  const int off_bars = off_P + 2 * XS_P_BYTES;
-  const int off_mx = off_bars + 256;             // [2 groups][2 halves][128] fp32 partial row maxima
-  auto q_full = [&](int s) { return bars + 8u * (0 + s); };
-  auto q_empty = [&](int s) { return bars + 8u * (2 + s); };
-  auto kv_full = [&](int s) { return bars + 8u * (4 + s); };
-  auto kv_empty = [&](int s) { return bars + 8u * (6 + s); };
-  auto s_full = [&](int s) { return bars + 8u * (8 + s); };
-  auto p_ready = [&](int s) { return bars + 8u * (10 + s); };
-  auto o_full = [&](int s) { return bars + 8u * (12 + s); };
-  const uint32_t tmem_slot = bars + 8u * 14;
-  volatile uint32_t* tmem_slot_g = reinterpret_cast<volatile uint32_t*>(gbase + off_bars + 8 * 14);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  // contiguous, balanced range of work items for this CTA
-  const int lo = (int)(((long long)p.total * blockIdx.x) / gridDim.x);
-  const int hi = (int)(((long long)p.total * (blockIdx.x + 1)) / gridDim.x);
-  const int n = hi - lo;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&p.tmQ);
-    tma_prefetch_desc(&p.tmK);
-    tma_prefetch_desc(&p.tmV);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(q_full(s), 1);
-      mbar_init(q_empty(s), 1);
-      mbar_init(kv_full(s), 1);
-      mbar_init(kv_empty(s), 1);
-      mbar_init(s_full(s), 1);
-      mbar_init(p_ready(s), 256);
-      mbar_init(o_full(s), 1);
-    }
-    mbar_fence_init();
-  }
-  if (warp == 2) tmem_alloc_rt(tmem_slot, 512u);
-  if (warp >= 2) {
-    // rows d..dN-1 of every V^T chunk are never written by TMA (its box has d rows): row d = ones, rest = 0
-    const int t = threadIdx.x - 64;
-    const int per_chunk = (dN - d) * 8;              // 16-byte granules
-    for (int i = t; i < 6 * per_chunk; i += XS_THREADS - 64) {
-      const int ch = i / per_chunk, g = i % per_chunk;
-      const uint32_t word = (g < 8) ? 0x3C003C00u : 0u;
-      *reinterpret_cast<uint4*>(gbase + off_V + ch * VC_BYTES + d * 128 + g * 16) = make_uint4(word, word, word, word);
-    }
-    fence_proxy_async_smem();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_g;
-  auto tS = [&](int g) { return tmem_base + (uint32_t)(g * XS_NKP); };
-  auto tO = [&](int g) { return tmem_base + (uint32_t)(2 * XS_NKP + g * dN); };
-  pdl_wait();                  // q is produced by the preceding projection GEMM
-  pdl_launch_dependents();
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int kvn = -1, prev_bh = -1;
-      for (int li = 0; li < n; ++li) {
-        const int item = lo + li;
-        const int bh = item / p.nqt, qt = item % p.nqt;
-        const int hb = bh % p.heads, bb = bh / p.heads;
-        if (bh != prev_bh) {
-          ++kvn;
-          prev_bh = bh;
-          const int ks = kvn & 1, ku = kvn >> 1;
-          if (ku >= 1) mbar_wait(kv_empty(ks), (ku - 1) & 1);     // every MMA that read the slot has completed
-          const int nvc = (p.Nk + 63) >> 6;                       // 64-key chunks of V^T that hold valid keys
-          mbar_expect_tx(kv_full(ks), XS_K_BYTES + nvc * d * 128);
-          tma_load_4d(sK + ks * XS_K_BYTES, &p.tmK, kv_full(ks), 0, 0, hb, bb);
-          for (int c = 0; c < nvc; ++c)
-            tma_load_4d(sV + ks * V_BYTES + c * VC_BYTES, &p.tmV, kv_full(ks), c * 64, 0, hb, bb);
-        }
-        const int qs = li & 1, qu = li >> 1;
-        if (qu >= 1) mbar_wait(q_empty(qs), (qu - 1) & 1);        // S of item li - 2 has read the slot
-        mbar_expect_tx(q_full(qs), XS_Q_BYTES);
-        tma_load_4d(sQ + qs * XS_Q_BYTES, &p.tmQ, q_full(qs), 0, qt * FA_BQ, hb, bb);
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc_s = make_idesc_f16(XS_NKP);
-      const uint32_t idesc_o = make_idesc_f16((uint32_t)dN);
-      const int ksteps_s = (d + 15) / 16;
-      const int ksteps_o = (p.Nk + 15) / 16;
-      int s_kvn = -1, s_prev = -1, o_kvn = -1, o_prev = -1;
-      auto issue_S = [&](int li) {
-        const int bh = (lo + li) / p.nqt;
-        if (bh != s_prev) {
-          ++s_kvn;
-          s_prev = bh;
-        }
-        const int g = li & 1, u = li >> 1;
-        mbar_wait(q_full(g), u & 1);
-        mbar_wait(kv_full(s_kvn & 1), (s_kvn >> 1) & 1);
-        tc_fence_after();
-        const uint64_t ad = make_sw128_kmajor_desc(sQ + g * XS_Q_BYTES);
-        const uint64_t bd = make_sw128_kmajor_desc(sK + (s_kvn & 1) * XS_K_BYTES);
-        for (int s = 0; s < ksteps_s; ++s) umma_f16(tS(g), ad + 2u * s, bd + 2u * s, idesc_s, s > 0 ? 1u : 0u);
-        umma_commit(s_full(g));
-        umma_commit(q_empty(g));
-      };
-      auto issue_PV = [&](int li) {
-        const int bh = (lo + li) / p.nqt;
-        if (bh != o_prev) {
-          ++o_kvn;
-          o_prev = bh;
-        }
-        const int g = li & 1, u = li >> 1;
-        mbar_wait(p_ready(g), u & 1);
-        tc_fence_after();
-        for (int s = 0; s < ksteps_o; ++s) {
-          const int c = s >> 2, k4 = s & 3;
-          const uint64_t ad = make_sw128_kmajor_desc(sP + g * XS_P_BYTES + c * (FA_BQ * 128));
-          const uint64_t bd = make_sw128_kmajor_desc(sV + (o_kvn & 1) * V_BYTES + c * VC_BYTES);
-          umma_f16(tO(g), ad + 2u * k4, bd + 2u * k4, idesc_o, s > 0 ? 1u : 0u);
-        }
-        umma_commit(o_full(g));
-        const bool last_of_head = (li + 1 == n) || ((lo + li + 1) / p.nqt != bh);
-        if (last_of_head) umma_commit(kv_empty(o_kvn & 1));
-      };
-      if (n > 0) issue_S(0);
-      if (n > 1) issue_S(1);
-      for (int li = 0; li < n; ++li) {
-        issue_PV(li);
-        if (li + 2 < n) issue_S(li + 2);
-      }
-    }
-  } else {
-    // ------------------------------------------------------------------ softmax / output groups (8 warps each)
-    // Two threads per query row: warps wi and wi + 4 of a group read the same TMEM lanes, thread `half` owns score
-    // columns [80 half, 80 half + 80) -> all of its logits sit in registers after ONE round of tcgen05.ld (no second
-    // pass over TMEM), 80 exponentials per thread per item, and 4 softmax warps per scheduler keep the MUFU pipe fed.
-    // The row maximum is exchanged through shared memory under a 256-thread named barrier.
-    const int g = (warp - 2) >> 3;
-    const int half = ((warp - 2) & 7) >> 2;
-    const int qd = warp & 3;                           // TMEM lane quarter this warp may access
-    const int row = qd * 32 + lane;
-    const uint32_t lane_off = static_cast<uint32_t>(qd * 32) << 16;
-    const float c2 = p.scale * 1.4426950408889634f;    // logits in log2 units
-    uint8_t* prow = gbase + off_P + g * XS_P_BYTES + row * 128;
-    const int rsw = row & 7;
-    const int cb = half * 80;                          // first score column of this thread
-    const int nvalid = min(max(p.Nk - cb, 0), 80);     // valid keys among its 80 columns
-    const int kcols = ((p.Nk + 15) >> 4) << 4;         // P columns the PV MMA reads
-    float* mxs = reinterpret_cast<float*>(gbase + off_mx) + g * 256;     // [half][row] partial row maxima
-    const uint32_t tSg = tS(g) + lane_off + cb, tOg = tO(g) + lane_off;
-    for (int li = g; li < n; li += 2) {
-      const int u = li >> 1;
-      const int item = lo + li;
-      const int bh = item / p.nqt, qt = item % p.nqt;
-      mbar_wait(s_full(g), u & 1);
-      tc_fence_after();
-      uint32_t r[80];
-      tmem_ld32(tSg, *reinterpret_cast<uint32_t(*)[32]>(&r[0]));
-      tmem_ld32(tSg + 32, *reinterpret_cast<uint32_t(*)[32]>(&r[32]));
-      tmem_ld16(tSg + 64, *reinterpret_cast<uint32_t(*)[16]>(&r[64]));
-      tmem_ld_wait();
-      if (nvalid < 80) {
-#pragma unroll
-        for (int i = 0; i < 80; ++i)
-          if (i >= nvalid) r[i] = 0xff800000u;          // -inf: masked keys contribute exp2(-inf) = 0
-      }
-      // exact row maximum: local (five independent 3-input max chains), then exchanged with the partner thread
-      float mx[5];
-#pragma unroll
-      for (int q = 0; q < 5; ++q) {
-        mx[q] = fmax3(__uint_as_float(r[q * 16]), __uint_as_float(r[q * 16 + 1]), __uint_as_float(r[q * 16 + 2]));
-#pragma unroll
-        for (int i = 3; i + 1 < 16; i += 2)
-          mx[q] = fmax3(mx[q], __uint_as_float(r[q * 16 + i]), __uint_as_float(r[q * 16 + i + 1]));
-        mx[q] = fmaxf(mx[q], __uint_as_float(r[q * 16 + 15]));
-      }
-      const float mloc = fmax3(fmax3(mx[0], mx[1], mx[2]), mx[3], mx[4]);
-      mxs[half * 128 + row] = mloc;
-      if (g == 0) asm volatile("bar.sync 1, 256;" ::: "memory");
-      else asm volatile("bar.sync 2, 256;" ::: "memory");
-      const float mrow = fmaxf(mloc, mxs[(half ^ 1) * 128 + row]);
-      const float nm = -mrow * c2;
-      // p = 2^(s * c2 - m) -> fp16 P in the K-major 128B-swizzled layout the PV MMA reads, 8 columns per granule
-#pragma unroll
-      for (int j = 0; j < 10; ++j) {
-        uint32_t pk[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float t0 = fmaf(__uint_as_float(r[8 * j + 2 * i]), c2, nm);
-          const float t1 = fmaf(__uint_as_float(r[8 * j + 2 * i + 1]), c2, nm);
-          if (PM == 1) {
-            const __half2 th = __floats2half2_rn(t0, t1);          // packed-half MUFU: two exponentials per op
-            pk[i] = ex2_f16x2(*reinterpret_cast<const uint32_t*>(&th));
-          } else if (PM > 1 && ((4 * j + i) % (PM > 1 ? PM : 2)) == (PM > 1 ? PM : 2) - 1) {
-            pk[i] = exp2_poly_h2(t0, t1);
-          } else {
-            const __half2 h = __floats2half2_rn(fast_exp2(t0), fast_exp2(t1));
-            pk[i] = *reinterpret_cast<const uint32_t*>(&h);
-          }
-        }
-        const int gc = cb + 8 * j;                      // first score column of this granule
-        if (gc < kcols)
-          *reinterpret_cast<uint4*>(prow + (gc >> 6) * (FA_BQ * 128) + ((((gc & 63) >> 3) ^ rsw) << 4)) =
-              make_uint4(pk[0], pk[1], pk[2], pk[3]);
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(p_ready(g));
-      // ---- epilogue of this item: O / l -> [B, Nq, heads*d]   (l = column d of the accumulator); the two threads
-      //      of a row take alternate 16-column chunks of O
-      mbar_wait(o_full(g), u & 1);
-      tc_fence_after();
-      const uint32_t lraw = tmem_ld1(tOg + d);
-      tmem_ld_wait();
-      const float l = __uint_as_float(lraw);
-      const float inv = l > 0.f ? 1.f / l : 0.f;
-      const int q = qt * FA_BQ + row;
-      const int b = bh / p.heads, h = bh % p.heads;
-      __half* orow = p.out + (long long)b * p.o_sb + (long long)q * p.o_sq + (long long)h * p.o_sh;
-      for (int c = half; c < (d + 15) / 16; c += 2) {
-        uint32_t o[16];
-        tmem_ld16(tOg + c * 16, o);
-        tmem_ld_wait();
-        if (q < p.Nq) {
-#pragma unroll
-          for (int h8 = 0; h8 < 2; ++h8) {
-            const int col = c * 16 + h8 * 8;
-            if (col < d) {
-              uint4 v;
-              __half2* hv = reinterpret_cast<__half2*>(&v);
-#pragma unroll
-              for (int i = 0; i < 4; ++i)
-                hv[i] = __floats2half2_rn(__uint_as_float(o[h8 * 8 + 2 * i]) * inv,
-                                          __uint_as_float(o[h8 * 8 + 2 * i + 1]) * inv);
-              *reinterpret_cast<uint4*>(orow + col) = v;
-            }
-          }
-        }
-      }
-      tc_fence_before();       // orders this item's TMEM reads before the arrive on p_ready of the next item
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_rt(tmem_base, 512u);
   }
 }
 
@@ -733,32 +319,29 @@ static int encode4d(CUtensorMap* m, const void* ptr, cuuint64_t inner, cuuint64_
   return 0;
 }
 
-template <int DCH, int PM>
+template <int DCH, int DP, int PM>
 static int launch_flash(const FlashParams& p, dim3 grid, cudaStream_t st) {
-  using Cfg = FlashCfg<DCH>;
+  using Cfg = FlashCfg<DCH, DP>;
   static bool done = false;
   if (!done) {
-    cudaError_t e = cudaFuncSetAttribute(flash_attn_kernel<DCH, PM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::smem_bytes(Cfg::DN));
-    if (e != cudaSuccess) return set_error("cudaFuncSetAttribute(flash DCH=%d): %s", DCH, cudaGetErrorString(e));
+    cudaError_t e = cudaFuncSetAttribute(flash_attn_kernel<DCH, DP, PM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         Cfg::SMEM_BYTES);
+    if (e != cudaSuccess) return set_error("cudaFuncSetAttribute(flash d<=%d): %s", DP, cudaGetErrorString(e));
     done = true;
   }
-  const int smem = Cfg::smem_bytes((p.d + 16) & ~15);
-  launch_k(flash_attn_kernel<DCH, PM>, grid, dim3(FA_THREADS), (size_t)smem, st, p);
+  launch_k(flash_attn_kernel<DCH, DP, PM>, grid, dim3(FA_THREADS), (size_t)Cfg::SMEM_BYTES, st, p);
   return check_launch("pfd_flash_attn_f16");
 }
 
-template <int PM>
-static int launch_xattn_short(const XsParams& p, int grid, int smem, cudaStream_t st) {
-  static bool done = false;
-  if (!done) {
-    cudaError_t e = cudaFuncSetAttribute(xattn_short_kernel<PM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         xs_smem_bytes(64));
-    if (e != cudaSuccess) return set_error("cudaFuncSetAttribute(xattn_short): %s", cudaGetErrorString(e));
-    done = true;
-  }
-  launch_k(xattn_short_kernel<PM>, dim3(grid), dim3(XS_THREADS), (size_t)smem, st, p);
-  return check_launch("pfd_flash_attn_f16(short keys)");
+template <int DP>
+static int launch_flash_pm(const FlashParams& p, dim3 grid, cudaStream_t st) {
+  // d <= 64 is MUFU-bound: a share of the exponentials may go to the FMA pipe ("flash_poly_mod": every n-th pair)
+  const int pm = option("flash_poly_mod", FLASH_POLY_MOD_DEFAULT);
+  if (pm == 1) return launch_flash<1, DP, 1>(p, grid, st);
+  if (pm == 2) return launch_flash<1, DP, 2>(p, grid, st);
+  if (pm == 3) return launch_flash<1, DP, 3>(p, grid, st);
+  if (pm == 4) return launch_flash<1, DP, 4>(p, grid, st);
+  return launch_flash<1, DP, 0>(p, grid, st);
 }
 
 }  // namespace pfd
@@ -776,29 +359,6 @@ extern "C" PFD_API int pfd_flash_attn_strided_f16(const void* q, const void* k, 
     if (q_strides[i] % 8 || k_strides[i] % 8 || vt_strides[i] % 8)
       return set_error("pfd_flash_attn_f16: strides must be multiples of 8 elements");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (Nk <= XS_NKP && d <= 48 && option("xattn_short", 1)) {
-    // cross-attention against a short context: persistent single-tile kernel (see xattn_short_kernel)
-    XsParams x;
-    memset(&x, 0, sizeof(x));
-    if (int rc = encode4d(&x.tmQ, q, d, Nq, heads, B, q_strides[2], q_strides[1], q_strides[0], FA_BQ, "Q")) return rc;
-    if (int rc = encode4d(&x.tmK, k, d, Nk, heads, B, k_strides[2], k_strides[1], k_strides[0], XS_NKP, "K")) return rc;
-    if (int rc = encode4d(&x.tmV, vt, Nk, d, heads, B, vt_strides[2], vt_strides[1], vt_strides[0], (cuuint32_t)d, "V^T")) return rc;
-    x.Nq = Nq; x.Nk = Nk; x.heads = heads; x.d = d;
-    x.nqt = (Nq + FA_BQ - 1) / FA_BQ;
-    const long long total = (long long)B * heads * x.nqt;
-    if (total > 0x7fffffffLL) return set_error("pfd_flash_attn_f16: problem too large");
-    x.total = (int)total;
-    x.scale = scale;
-    x.out = static_cast<__half*>(out);
-    x.o_sb = o_sb; x.o_sq = o_sq; x.o_sh = d;
-    const int sms = num_sms();
-    const int grid = x.total < sms ? x.total : sms;
-    const int smem = xs_smem_bytes((d + 16) & ~15);
-    const int pm = option("flash_poly_mod", FLASH_POLY_MOD_DEFAULT);
-    if (pm == 4) return launch_xattn_short<4>(x, grid, smem, st);
-    if (pm == 1) return launch_xattn_short<1>(x, grid, smem, st);
-    return launch_xattn_short<0>(x, grid, smem, st);
-  }
   FlashParams p;
   memset(&p, 0, sizeof(p));
   // strides = {batch, head, row} in elements; q/k rows run over d, vt rows (one per channel) run over the keys
@@ -811,17 +371,20 @@ extern "C" PFD_API int pfd_flash_attn_strided_f16(const void* q, const void* k, 
   p.out = static_cast<__half*>(out);
   p.o_sb = o_sb; p.o_sq = o_sq; p.o_sh = d;
   dim3 grid((Nq + FA_BQ - 1) / FA_BQ, (unsigned)((long long)B * heads));
-  if (d <= 64) {
-    // d <= 64 is MUFU-bound: a share of the exponentials goes to the FMA pipe ("flash_poly_mod": every n-th pair)
-    const int pm = option("flash_poly_mod", FLASH_POLY_MOD_DEFAULT);
-    if (pm == 1) return launch_flash<1, 1>(p, grid, st);
-    if (pm == 2) return launch_flash<1, 2>(p, grid, st);
-    if (pm == 3) return launch_flash<1, 3>(p, grid, st);
-    if (pm == 4) return launch_flash<1, 4>(p, grid, st);
-    return launch_flash<1, 0>(p, grid, st);
+  switch ((d + 15) / 16) {
+    case 1: return launch_flash_pm<16>(p, grid, st);
+    case 2: return launch_flash_pm<32>(p, grid, st);
+    case 3: return launch_flash_pm<48>(p, grid, st);
+    case 4: return launch_flash_pm<64>(p, grid, st);
+    case 5: return launch_flash<2, 80, 0>(p, grid, st);
+    case 6: return launch_flash<2, 96, 0>(p, grid, st);
+    case 7: return launch_flash<2, 112, 0>(p, grid, st);
+    case 8: return launch_flash<2, 128, 0>(p, grid, st);
+    case 9: return launch_flash<3, 144, 0>(p, grid, st);
+    case 10: return launch_flash<3, 160, 0>(p, grid, st);
+    case 11: return launch_flash<3, 176, 0>(p, grid, st);
+    default: return launch_flash<3, 192, 0>(p, grid, st);
   }
-  if (d <= 128) return launch_flash<2, 0>(p, grid, st);
-  return launch_flash<3, 0>(p, grid, st);
 }
 
 extern "C" PFD_API int pfd_flash_attn_f16(const void* q, const void* k, const void* vt, void* out, int32_t B,

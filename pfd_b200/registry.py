@@ -4,7 +4,7 @@ Mirrors lib/model_zoo/common/get_model.py:32-124 (`get_model()` singleton, `@reg
 `get_model()(cfg)` with cfg.type / cfg.args / cfg.pth|pretrained / strict_sd) and the part of
 lib/cfg_helper.py:102-146 that app.py uses (`model_cfg_bank()(name)`).  `install_into_reference()`
 registers the pfd_b200 classes under the reference's own type names inside the reference's registry,
-so `app.py` (run from the reference tree) builds the B200 pipeline unchanged — see INTEGRATION.md.
+so `app.py` (run from the reference tree) builds the pfd_b200 pipeline unchanged — see INTEGRATION.md.
 """
 from __future__ import annotations
 

@@ -1,8 +1,8 @@
 """The reference-facing boundary (SURVEY.md §8b): `pfd_b200.install_into_reference()` registers the pfd_b200 classes
 in the REFERENCE's own registry, so the reference's `model_cfg_bank` / `get_model` (what app.py calls, app.py:111)
-build the B200 pipeline, and reference-built state dicts load with strict=True (app.py:137-162).
+build the pfd_b200 pipeline, and reference-built state dicts load with strict=True (app.py:137-162).
 
-Needs the reference tree (/root/reference in the build container, or its staged copy baseline/_ref); skipped otherwise.
+Needs the reference tree (its copy staged under oracle/_ref by build(), or PFD_REFERENCE); skipped otherwise.
 Runs in a child process because the harness chdir()s into the reference tree and patches sys.modules."""
 import json
 import os
@@ -61,7 +61,7 @@ print("RESULT " + json.dumps(res))
 def test_install_into_reference_builds_pfd_b200_through_the_reference_registry():
     import ref_harness as rh
     if not rh.available():
-        pytest.skip("reference tree not present (/root/reference or baseline/_ref)")
+        pytest.skip("reference tree not present (oracle/_ref or PFD_REFERENCE)")
     r = subprocess.run([sys.executable, "-c", CHILD, ROOT], capture_output=True, text=True, timeout=900,
                        env=dict(os.environ, CUDA_VISIBLE_DEVICES=""))
     assert r.returncode == 0, r.stderr[-3000:]

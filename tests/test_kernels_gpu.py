@@ -68,12 +68,11 @@ def test_linear_two_segments(nv):
 
 @pytest.mark.parametrize("case", ["linear_res", "linear_narrow", "linear_ragged", "linear_slice", "conv_res", "conv_small",
                                   "conv_rowadd_silu", "conv_stride2", "bmm"])
-def test_gemm_tma_store_epilogue_bit_exact(nv, case):
-    """The TMA-store epilogue (tile staged in swizzled shared-memory slabs, residual TMA-loaded into the same slabs,
-    cp.async.bulk.tensor stores, clipping by the TMA unit) must produce EXACTLY the bits of the register epilogue
-    (option gemm_tma_epi = 0) - same fp32 math, same fp16 rounding points - for every raster tiling: 128x1x1 rows
-    (Linear), 8x8x2 / 16x8 / 32x4 pixel tiles (convs), ragged rows / columns, N not a multiple of the tile, an output
-    that is a column slice of a wider tensor, per-image row add + activation, and batched B."""
+def test_gemm_epilogue_rasters(nv, case):
+    """The GEMM epilogue for every raster tiling: 128x1x1 rows (Linear), 8x8x2 / 16x8 / 32x4 pixel tiles (convs),
+    ragged rows / columns, N not a multiple of the tile, an output that is a column slice of a wider tensor (the
+    columns outside the slice stay untouched), per-image row add + activation, and batched B.  Against torch fp32,
+    and a second launch must reproduce the bits."""
     def run():
         if case == "linear_res":
             x, w, b, r = rnd(4096, 320), rnd(320, 320, scale=320 ** -0.5, seed=1), rnd(320, seed=2), rnd(4096, 320, seed=3)
@@ -115,30 +114,20 @@ def test_gemm_tma_store_epilogue_bit_exact(nv, case):
         nv.gemm_raw([(q, 1, 64, (64, 64 * 200, 64 * 200))], in_w=200, in_h=1, stride=1, W=200, H=1, NB=6, w=k, N=136, K=64,
                     b_batch_stride=136 * 64, out=s_, so=(200 * 136, 0, 0, 136, 0, 1))
         return s_, torch.bmm(q.float(), k.float().transpose(1, 2))
-    nv.set_env_option(None, None)
-    try:
-        nv.set_env_option("gemm_streamk", 0)        # the stream-K tail changes the fp32 summation order (own test below)
-        nv.set_env_option("gemm_tma_epi", 0)
-        out0, ref = run()
-        out0 = out0.clone()
-        nv.set_env_option("gemm_tma_epi", 1)
-        out1, _ = run()
-        torch.cuda.synchronize()
-    finally:
-        nv.set_env_option(None, None)
+    out0, ref = run()
+    out0 = out0.clone()
+    out1, _ = run()
+    torch.cuda.synchronize()
     close(out0, ref)
-    assert torch.equal(out0, out1), f"TMA-store epilogue differs from the register epilogue: max |d| = {(out0.float() - out1.float()).abs().max().item()}"
+    assert torch.equal(out0, out1), f"two launches differ: max |d| = {(out0.float() - out1.float()).abs().max().item()}"
 
 
 @pytest.mark.parametrize("case", ["conv_res_2tiles", "conv_many_waves", "conv_wide_rowadd_silu", "linear_odd_ragged",
                                   "conv_stride2", "conv_tiny", "conv_skip_segments"])
-def test_gemm_cta_pair(nv, case):
-    """CTA-pair kernel (cluster of two, tcgen05 cta_group::2: M = 256 across the pair, B split between the two CTAs,
-    cta_group::2 TMA loads completing on the leader's barrier, multicast commits, remote tmem_empty arrives) against
-    torch fp32 and against the single-CTA kernel on the same operands.  Cases: one / many tiles per cluster (accumulator
-    double buffering and pipeline phases across tiles), BN = 256 / 160 / 128, an ODD number of 128-row tiles (the
-    second CTA of the last pair works on a tile that is completely outside the raster), N not a multiple of the
-    tile, stride 2, per-image row add + SiLU, residual, extra 1x1 K segments."""
+def test_gemm_conv_tilings(nv, case):
+    """Long-K convs and Linears against torch fp32: one / many tiles per CTA of the persistent kernel (pipeline phases
+    across tiles), N tiles 256 / 160 / 128, an odd number of 128-row tiles, N not a multiple of the tile, stride 2,
+    per-image row add + SiLU, residual, extra 1x1 K segments."""
     def run():
         if case == "linear_odd_ragged":
             x, w, r = rnd(640, 1024), rnd(1288, 1024, scale=1024 ** -0.5, seed=1), rnd(640, 1288, seed=3)
@@ -169,28 +158,16 @@ def test_gemm_cta_pair(nv, case):
             out = nv.conv3x3(x, wp, b, residual=r)
             ref = F.conv2d(xr, w4.float(), b.float(), padding=1) + r.float().permute(0, 3, 1, 2)
         return out, ref.permute(0, 2, 3, 1)
-    nv.set_env_option(None, None)
-    try:
-        nv.set_env_option("gemm_pair", 0)
-        out0, ref = run()
-        out0 = out0.clone()
-        nv.set_env_option("gemm_pair", 2)          # 2 = force the pair kernel wherever it is applicable
-        out1, _ = run()
-        torch.cuda.synchronize()
-    finally:
-        nv.set_env_option(None, None)
-    close(out0, ref)
-    close(out1, ref)
-    dmax = (out0.float() - out1.float()).abs().max().item()
-    print(f"[cta pair] {case}: max |pair - single| = {dmax:.3e}")
-    assert dmax <= 2e-3 * max(1.0, ref.abs().max().item())
+    out, ref = run()
+    torch.cuda.synchronize()
+    close(out, ref)
 
 
 @pytest.mark.parametrize("case", ["conv_l1", "conv_l2_single_wave", "conv_l0_res", "linear_bigk_res", "conv_ragged_rowadd_silu"])
 def test_gemm_stream_k_tail(nv, case):
     """Stream-K tail of the persistent GEMM: the tiles of the last, partially filled wave are cut into K ranges over ALL
     SMs (contributors publish fp32 partial tiles through the workspace + a ready flag, the CTA that reaches the tile's
-    last K block adds them and runs the normal TMA-store epilogue).  Against torch fp32 and against the plain tiling
+    last K block adds them and runs the normal epilogue).  Against torch fp32 and against the plain tiling
     (gemm_streamk = 0; only the fp32 summation order differs); each case is launched three times and replayed from a
     CUDA graph, which must give identical bits (the flags are reset by their consumers)."""
     if case == "linear_bigk_res":
@@ -473,11 +450,10 @@ def test_flash_attention(nv, B, heads, Nq, Nk, d):
                                              (1, 2, 300, 77, 40), (2, 3, 130, 160, 48), (1, 5, 257, 20, 8),
                                              (1, 1, 128, 33, 16), (2, 8, 9216, 148, 40)])
 def test_short_key_attention(nv, B, heads, Nq, Nk, d):
-    """Cross-attention against a short context (Nk <= 160, d <= 48): the persistent single-score-tile kernel
-    (xattn_short_kernel: contiguous (batch*head, query tile) ranges per CTA, K / V^T resident per head, two softmax
-    groups) against an fp32 torch reference and against the generic flash kernel on the same operands.  Shapes cover
-    the BASELINE level-0 launches (512x512: 4096 queries, 768x768: 9216), ragged query counts, one query tile per
-    head (a K / V^T reload for every item), partial / full last key chunk and the smallest head dims."""
+    """Cross-attention against a short context (Nk <= 160, d <= 48) through the flash kernel against an fp32 torch
+    reference.  Shapes cover the BASELINE level-0 launches (512x512: 4096 queries, 768x768: 9216), ragged query
+    counts, one query tile per head, partial / full last key block and the smallest head dims; one launch per call,
+    a finite output everywhere (the output starts as NaN) and a relative rms error of at most 1.5e-3."""
     g = torch.Generator().manual_seed(Nq + Nk)
     q = torch.randn((B * heads, Nq, d), generator=g).cuda().half()
     Nkp = (Nk + 7) // 8 * 8
@@ -487,16 +463,10 @@ def test_short_key_attention(nv, B, heads, Nq, Nk, d):
     vt[:, :, :Nk] = torch.randn((B * heads, d, Nk), generator=g).cuda().half()
     scale = d ** -0.5
     out_s = torch.full((B, Nq, heads * d), float("nan"), device="cuda", dtype=torch.float16)
-    out_f = torch.empty_like(out_s)
     nv.set_env_option(None, None)
     n0 = nv.launch_count()
     nv.flash_attn(q, k, vt, B=B, heads=heads, Nq=Nq, Nk=Nk, scale=scale, out=out_s)
     assert nv.launch_count() == n0 + 1
-    try:
-        nv.set_env_option("xattn_short", 0)
-        nv.flash_attn(q, k, vt, B=B, heads=heads, Nq=Nq, Nk=Nk, scale=scale, out=out_f)
-    finally:
-        nv.set_env_option(None, None)
     torch.cuda.synchronize()
     s = (torch.bmm(q.float(), k[:, :Nk].float().transpose(1, 2)).half().float() * scale).half().float()
     ref = torch.bmm(torch.softmax(s, -1), vt[:, :, :Nk].float().transpose(1, 2))
@@ -504,9 +474,8 @@ def test_short_key_attention(nv, B, heads, Nq, Nk, d):
     assert torch.isfinite(out_s.float()).all()
     close(out_s, ref, rtol=8e-3, atol=4e-3)
     es = ((out_s.float() - ref).pow(2).mean() / ref.pow(2).mean()).sqrt().item()
-    ef = ((out_f.float() - ref).pow(2).mean() / ref.pow(2).mean()).sqrt().item()
-    print(f"[short-key attention] B={B} h={heads} {Nq}x{Nk} d={d}: rel rms short {es:.2e}  generic flash {ef:.2e}")
-    assert es < max(1.5 * ef, 1.5e-3)
+    print(f"[short-key attention] B={B} h={heads} {Nq}x{Nk} d={d}: rel rms {es:.2e}")
+    assert es < 1.5e-3
 
 
 @pytest.mark.parametrize("B,heads,N,d", [(2, 8, 4096, 40), (2, 8, 1024, 80), (1, 8, 256, 160), (3, 4, 64, 40)])

@@ -191,5 +191,5 @@ def test_config_fixture_is_complete(cgold):
     need = ["c1_ctx", "c1_latent", "c1_image", "c2_eps_t981", "c2_eps_t501", "c2_eps_t1", "c3_eps", "c4_eps",
             "c5_ctx", "c5_x_step0", "c5_x_step1", "c6_ctx", "c7_latent", "c8_mean", "c8_logvar", "c9_latent"]
     assert all(k in cgold for k in need), [k for k in need if k not in cgold]
-    assert cgold["c2_eps_t501"].shape == (8, 4, 64, 64) and cgold["c5_x_step1"].shape == (1, 4, 96, 96)
-    assert cgold["c1_image"].shape == (1, 3, 512, 512)
+    assert tuple(cgold["c2_eps_t501__shape"]) == (8, 4, 64, 64) and tuple(cgold["c5_x_step1__shape"]) == (1, 4, 96, 96)
+    assert tuple(cgold["c1_image__shape"]) == (1, 3, 512, 512) and cgold["c5_x_step0"].shape == (1, 4, 96, 96)

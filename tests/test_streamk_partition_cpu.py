@@ -1,5 +1,5 @@
 """Host-side model of the stream-K work partition of the persistent GEMM (pfd_b200/csrc/gemm_tc.cu: sk_range /
-gemm_work<true> / the owner's contributor scan in tma_store_epilogue): the arithmetic is restated here 1:1 and checked
+gemm_work<true> / the owner's contributor scan in sk_gather): the arithmetic is restated here 1:1 and checked
 exhaustively over the tile counts, grid sizes and K depths the library can select, for the properties the device code
 relies on.  (The device code itself is exercised by tests/test_kernels_gpu.py::test_gemm_stream_k_tail.)
 
@@ -42,7 +42,7 @@ def gemm_work(c, wi, G, dp_tiles, R, KB):
 
 
 def owner_sources(c, t, G, R, KB):
-    """Contributor slots found by the owner's backwards scan (tma_store_epilogue, sk_mode == 2)."""
+    """Contributor slots found by the owner's backwards scan (sk_gather, mode 2)."""
     tstart = t * KB
     out = []
     cc = c - 1

@@ -2,8 +2,6 @@
 settings INSIDE ONE PROCESS, interleaved, so that box-to-box spread and the power/thermal state do not bias the
 comparison (r2: three separate bench.py runs on one box disagreed by 4 % in the opposite direction of their own
 per-kernel breakdowns).  Each variant is captured into its own CUDA graph; rounds alternate between the graphs.
-profiles/r2_ab_unet_ew16_producer_stats.log is the run that rejected the 16-epilogue-warp GEMM variant and the
-producer-side GroupNorm statistics (both removed again).
 
     python tools/ab_unet.py [--rounds 6] [--reps 20] [--control] [--env-variant name=option:value ...]
 """

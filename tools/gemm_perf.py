@@ -1,4 +1,4 @@
-"""Per-shape throughput of the tcgen05 GEMM / implicit-GEMM conv kernel and the flash attention
+"""Per-shape throughput of the wgmma GEMM / implicit-GEMM conv kernel and the flash attention
 kernel on the UNet's hot shapes (CUDA events, 3 warm-up + 10 timed launches, inputs >> L2 not enforced:
 the same operands are reused, so these are L2-warm kernel rates; bench.py measures the cold-ish pipeline)."""
 import json

@@ -47,6 +47,26 @@ def sub(t, stride):
     return t.detach().float().reshape(-1)[::stride].numpy().astype(np.float32)
 
 
+# Tensors the tests feed back into the pipeline (teacher forcing, decode of the reference latent, the posterior
+# formula) are stored whole; every other tensor is only compared, so a fixed strided sample of at most
+# SAMPLE_MAX elements is stored with its full shape under "<key>__shape" (keeps the file under 1 MB).
+FULL_KEYS = ("c1_latent", "c5_ctx", "c5_x_step0", "c7_latent", "c8_mean", "c8_logvar", "c9_latent")
+SAMPLE_MAX = 4096
+
+
+def sample_for_storage(out):
+    res = {}
+    for k, v in out.items():
+        if k.endswith("__shape") or k in FULL_KEYS:
+            res[k] = v
+            continue
+        v = np.asarray(v)
+        stride = -(-v.size // SAMPLE_MAX)
+        res[k] = v.reshape(-1)[::stride].astype(np.float32)
+        res[k + "__shape"] = np.asarray(v.shape, dtype=np.int64)
+    return res
+
+
 def main():
     cases = sys.argv[1:] or ["c1", "c2", "c3", "c4", "c5", "c6", "c7", "c8", "c9"]
     torch.set_grad_enabled(False)
@@ -172,7 +192,7 @@ def main():
         out["c9_latent"] = x.numpy().astype(np.float32)
         print(f"c9: latent rms {x.pow(2).mean().sqrt():.3f}", flush=True)
 
-    np.savez_compressed(OUT, **out)
+    np.savez_compressed(OUT, **sample_for_storage(out))
     print(f"wrote {OUT} ({os.path.getsize(OUT) / 1e6:.2f} MB) in {time.time() - t0:.0f}s", flush=True)
 
 

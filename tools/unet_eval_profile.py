@@ -1,6 +1,6 @@
 """One CFG-pair UNet evaluation (batch 4 -> 8 rows, 64x64 latents) run eagerly twice: meant to be run under
 `ncu --metrics gpu__time_duration.sum --cache-control none --clock-control none` with PFD_GEMM_TRACE=1 so that
-tools/gemm_breakdown.py can join the per-launch device times with the GEMM call descriptors."""
+the per-launch device times can be joined with the GEMM call descriptors."""
 import os
 import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
