@@ -793,6 +793,17 @@ extern "C" PFD_API int pfd_gemm_f16(const pfd_gemm_desc* d) {
   const long long m_tiles = (long long)p.tiles_w * p.tiles_h * p.tiles_nb;
 
   // ---- N tile: minimise (waves x per-tile cost)
+  // Plain GEMMs with short K (every segment 1x1, at most 40 K blocks of 64, one B for all rows) take 128 x 64 tiles.
+  // There a tile's time grows much faster than its width, so the wave model below ranks the wide tiles too well:
+  // on H100 the UNet's K = 320 ... 2560 Linears run 1.2x to 1.6x faster with 64-wide than with the 160-wide tiles it
+  // picks (tools/gemm_sweep.py).  Longer K (convolutions, K = 5120) keeps the model.
+  bool short_k_plain = !p.b_batched && !geglu;
+  int kb_count = 0;
+  for (int s = 0; s < d->nseg; ++s) {
+    if (d->taps[s] != 1) short_k_plain = false;
+    kb_count += d->taps[s] * ((d->a_c[s] + BK - 1) / BK);
+  }
+  short_k_plain = short_k_plain && kb_count <= 40;
   const int cands[5] = {256, 192, 160, 128, 64};
   int BNsel = 128;
   double best_cost = -1;
@@ -801,6 +812,7 @@ extern "C" PFD_API int pfd_gemm_f16(const pfd_gemm_desc* d) {
     const int bn_c = cands[i];
     if (geglu && (d->N % bn_c)) continue;
     if (d->bn_force && d->bn_force != bn_c) continue;
+    if (short_k_plain && !d->bn_force && bn_c != 64) continue;
     const long long nt = cdivll(d->N, bn_c);
     const long long tiles = m_tiles * nt;
     const double waves = (double)cdivll(tiles, sms);
