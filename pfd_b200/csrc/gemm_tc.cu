@@ -4,11 +4,15 @@
 //
 //   D[128 x BN] (fp32, registers)  +=  A[128 x 64] (fp16, smem, TMA 4-D box)  x  B[BN x 64]^T (fp16, smem)
 //
-// Roles (384 threads): warpgroup 0 = TMA producer (one thread), warpgroups 1 and 2 = wgmma consumers, each owning
-// 64 rows of the tile, followed by the fused epilogue (bias / time-embedding / activation / GEGLU / residual ->
-// global) straight from the accumulator registers.  The producer runs ahead through a ring of shared-memory stages,
-// so the loads of tile i+1 overlap the epilogue of tile i.  See include/pfd_b200.h (pfd_gemm_f16) for the reference
-// call sites this replaces.
+// Roles (384 threads): warpgroup 0 = TMA producer (thread 0) and three store warps (warps 1-3); warpgroups 1 and 2 =
+// wgmma consumers, each owning 64 rows of the tile.  After a tile's MMAs the consumers apply the fused epilogue
+// (bias / time-embedding / activation / GEGLU) and write the fp16 tile to a shared-memory staging buffer, then go on
+// to the next tile's K blocks; the store warps add the residual and write the tile to global memory with 16-byte
+// stores while those MMAs run (gemm_stage_tile / gemm_store_tile, barriers c_full / c_empty).  Split-K partials and
+// element-strided outputs keep the direct epilogue from the registers (gemm_epilogue); stream-K contributors hand
+// their fp32 partial tile to the owner, whose epilogue is staged.  The producer runs ahead through a ring of
+// shared-memory stages, so the loads of tile i+1 overlap the epilogue of tile i.  See include/pfd_b200.h
+// (pfd_gemm_f16) for the reference call sites this replaces.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -66,16 +70,30 @@ struct alignas(64) GemmParams {
   int vec_ok;
 };
 
+constexpr int STORE_THREADS = 96;           // warps 1-3 of the producer warpgroup
+
 template <int BN>
 struct GemmCfg {
   static constexpr int STAGE_B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = STAGE_A_BYTES + STAGE_B_BYTES;
-  static constexpr int RAW_STAGES = (SMEM_BUDGET - SMEM_FIXED) / STAGE_BYTES;
+  // staged fp16 output tile: rows padded by 16 B, so the 8 rows x 4 lanes of a warp's half2 fragment writes fall on
+  // 32 distinct banks; followed by the store warps' output row offsets of two consecutive tiles
+  static constexpr int C_PITCH = BN * 2 + 16;
+  static constexpr int C_BYTES = BM * C_PITCH + 2 * BM * 8;
+  static constexpr int RAW_STAGES = (SMEM_BUDGET - SMEM_FIXED - C_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = RAW_STAGES > 8 ? 8 : RAW_STAGES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + SMEM_FIXED;
+  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + C_BYTES + SMEM_FIXED;
+  // Register budgets (setmaxnreg) of the two roles.  The CTA starts with 168 per thread (__launch_bounds__(384, 1)),
+  // so 128 PRODUCER_REGS + 256 CONSUMER_REGS = 384 x 168.  The producer warpgroup's budget bounds the store warps'
+  // STORE_BATCH (16-byte chunks per thread whose residual loads are in flight at once); the 256-wide tile's consumers
+  // (128 fp32 accumulators) need more than 216 registers with the stream-K gather.
+  static constexpr int CONSUMER_REGS = BN >= 256 ? 224 : 208;
+  static constexpr int PRODUCER_REGS = BN >= 256 ? 56 : 88;
+  static constexpr int STORE_BATCH = BN >= 256 ? 4 : 8;
+  static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS == GEMM_THREADS * 168, "register budgets");
   static_assert(STAGE_B_BYTES % 1024 == 0, "B stage must keep 1024-B swizzle alignment");
   static_assert(BN % 16 == 0 && BN >= 16 && BN <= 256, "wgmma N constraint");
-  static_assert(STAGES >= 3, "too few pipeline stages");
+  static_assert(STAGES == (BN <= 64 ? 8 : BN <= 160 ? 5 : BN <= 192 ? 4 : 3), "pipeline depth per N tile");
 };
 
 // erf to ~1.5e-7 absolute (Abramowitz & Stegun 7.1.26) with MUFU rcp/ex2: about half the
@@ -260,27 +278,208 @@ __device__ __forceinline__ void sk_gather(const GemmParams& p, float (&acc)[BN /
   }
 }
 
-// Epilogue of one consumer warpgroup: rows [64 cw, 64 cw + 64) of the tile straight from the wgmma accumulator
-// fragment.  Thread (warp wl, lane l) holds rows 16 wl + l/4 (+ 8) and, for every 8-column group j, the column pair
-// 8j + 2 (l % 4) (+ 1): acc[4j + {0, 1}] for the first row, acc[4j + {2, 3}] for the second.
+// Position of a tile row in the output raster: (x, y, image n) and whether it lies inside the raster.
+struct TileRow {
+  int x, y, n;
+  bool valid;
+};
+__device__ __forceinline__ TileRow tile_row(const GemmParams& p, int m_tile, int row) {
+  const int tx = m_tile % p.tiles_w;
+  const int ty = (m_tile / p.tiles_w) % p.tiles_h;
+  const int tn = m_tile / (p.tiles_w * p.tiles_h);
+  TileRow r;
+  r.x = tx * p.bw + row % p.bw;
+  r.y = ty * p.bh + (row / p.bw) % p.bh;
+  r.n = tn * p.bn + row / (p.bw * p.bh);
+  r.valid = (r.x < p.W) && (r.y < p.H) && (r.n < p.NB);
+  return r;
+}
+__device__ __forceinline__ long long out_row_off(const GemmParams& p, const TileRow& r) {
+  return (long long)(r.n / p.ndiv) * p.so_n1 + (long long)(r.n % p.ndiv) * p.so_n0 + (long long)r.y * p.so_y +
+         (long long)r.x * p.so_x;
+}
+__device__ __forceinline__ long long out_col_off(const GemmParams& p, int c) {
+  return p.cdiv >= p.N ? (long long)c * p.so_c0 : (long long)(c / p.cdiv) * p.so_c1 + (long long)(c % p.cdiv) * p.so_c0;
+}
+
+// Accumulator fragment of a consumer warpgroup (rows [64 cw, 64 cw + 64) of the tile): thread (warp wl, lane l) holds
+// rows 16 wl + l/4 (+ 8) and, for every 8-column group j, the column pair 8j + 2 (l % 4) (+ 1): acc[4j + {0, 1}] for
+// the first row, acc[4j + {2, 3}] for the second.
+//
+// Staged epilogue (every tile with 16-byte addressable output columns, vec_ok, and no split-K): the consumers write
+// the tile's fp16 values into the shared-memory buffer `cbuf` (row pitch C_PITCH) and go on to the next tile; the
+// store warps (gemm_store_tile) add the residual and write the rows to global memory.
+//   * GEGLU (tile packed [value(BN/2) | gate(BN/2)], pack_geglu): fp16(value) * fp16(gelu(fp16(gate))) in columns
+//     [0, BN/2) of the buffer;
+//   * otherwise fp16(act(acc * alpha + bias + row add)).
+// The bias and row-add loads of a block of column groups are all issued before any of them is used.
+template <int BN>
+__device__ __forceinline__ void gemm_stage_tile(const GemmParams& p, const float (&acc)[BN / 2], int cw, int tile,
+                                                uint8_t* cbuf) {
+  constexpr int C_PITCH = GemmCfg<BN>::C_PITCH;
+  const int wl = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const int n_tile = tile % p.n_tiles;
+  const int m_tile = tile / p.n_tiles;
+  const bool geglu = (p.act == PFD_ACT_GEGLU);
+  const int n_out = geglu ? p.N / 2 : p.N;
+  const int col_base = n_tile * (geglu ? BN / 2 : BN);
+  const int cq = 2 * (lane & 3);
+  int rows[2];
+  bool valid[2];
+  const __half* rowadd_row[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    rows[i] = cw * 64 + wl * 16 + (lane >> 2) + 8 * i;
+    const TileRow r = tile_row(p, m_tile, rows[i]);
+    valid[i] = r.valid;
+    rowadd_row[i] = (p.rowadd && r.valid) ? p.rowadd + (long long)r.n * p.rowadd_ld : nullptr;
+  }
+  auto put = [&](int i, int c, __half2 h) {
+    *reinterpret_cast<__half2*>(cbuf + rows[i] * C_PITCH + c * 2) = h;
+  };
+  const float alpha = p.alpha;
+  if (geglu) {
+    uint32_t bv[BN / 16], bg[BN / 16];
+#pragma unroll
+    for (int j = 0; j < BN / 16; ++j) {
+      const int c = 8 * j + cq;
+      const bool ld = p.bias && col_base + c < n_out;
+      bv[j] = ld ? ldg_h2(p.bias + (long long)n_tile * BN + c) : 0u;
+      bg[j] = ld ? ldg_h2(p.bias + (long long)n_tile * BN + BN / 2 + c) : 0u;
+    }
+#pragma unroll
+    for (int j = 0; j < BN / 16; ++j) {
+      const int c = 8 * j + cq;               // value column inside the tile; its gate is column c + BN / 2
+      if (col_base + c >= n_out) continue;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        if (!valid[i]) continue;
+        const float* v = &acc[4 * j + 2 * i];
+        const float* g = &acc[4 * (j + BN / 16) + 2 * i];
+        // reference: x, gate = proj(x).chunk(2) are fp16 tensors; x * gelu(gate) in fp16 (attention.py:50-51)
+        const __half2 a = __floats2half2_rn(fmaf(v[0], alpha, h2lo(bv[j])), fmaf(v[1], alpha, h2hi(bv[j])));
+        const float2 gf = __half22float2(__floats2half2_rn(fmaf(g[0], alpha, h2lo(bg[j])), fmaf(g[1], alpha, h2hi(bg[j]))));
+        put(i, c, __hmul2(a, __floats2half2_rn(gelu_sig(gf.x), gelu_sig(gf.y))));
+      }
+    }
+    return;
+  }
+  const int act = p.act;
+  constexpr int JB = (BN / 8) % 8 == 0 ? 8 : 4;   // column groups per block of loads
+#pragma unroll
+  for (int j0 = 0; j0 < BN / 8; j0 += JB) {
+    uint32_t bb[JB], ra[2][JB];
+#pragma unroll
+    for (int jj = 0; jj < JB; ++jj) {
+      const int col = col_base + 8 * (j0 + jj) + cq;
+      const bool in = col < n_out;
+      bb[jj] = (p.bias && in) ? ldg_h2(p.bias + col) : 0u;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) ra[i][jj] = (rowadd_row[i] && in) ? ldg_h2(rowadd_row[i] + col) : 0u;
+    }
+#pragma unroll
+    for (int jj = 0; jj < JB; ++jj) {
+      const int j = j0 + jj;
+      if (col_base + 8 * j + cq >= n_out) continue;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        if (!valid[i]) continue;
+        float v0 = fmaf(acc[4 * j + 2 * i], alpha, h2lo(bb[jj]));
+        float v1 = fmaf(acc[4 * j + 2 * i + 1], alpha, h2hi(bb[jj]));
+        if (rowadd_row[i]) {
+          // per-image row add (time embedding): (conv + bias) + emb -> act, the reference's order
+          v0 += h2lo(ra[i][jj]);
+          v1 += h2hi(ra[i][jj]);
+        }
+        if (act != PFD_ACT_NONE) {
+          v0 = act_apply(v0, act);
+          v1 = act_apply(v1, act);
+        }
+        put(i, 8 * j + cq, __floats2half2_rn(v0, v1));
+      }
+    }
+  }
+}
+
+// Store warps (warps 1-3 of warpgroup 0): write one staged tile from `cbuf` to its output rows in 16-byte chunks and
+// add the residual in fp16 - the reference's `x + f(h)` on fp16 tensors.  A quarter-warp reads 128 contiguous bytes
+// of the buffer.  The output row offsets are computed first (`rowoff`, one of two buffers used by alternate tiles);
+// then each thread issues the residual loads of STORE_BATCH chunks before any of their stores.  The first batch is
+// loaded before waiting for the consumers to fill the buffer (`c_full`, phase `parity`).
+template <int BN>
+__device__ __forceinline__ void gemm_store_tile(const GemmParams& p, int tile, const uint8_t* cbuf, long long* rowoff,
+                                                uint32_t c_full, uint32_t parity) {
+  constexpr int C_PITCH = GemmCfg<BN>::C_PITCH;
+  constexpr int STORE_BATCH = GemmCfg<BN>::STORE_BATCH;
+  const int t = threadIdx.x - 32;
+  const int n_tile = tile % p.n_tiles;
+  const int m_tile = tile / p.n_tiles;
+#pragma unroll 1
+  for (int row = t; row < BM; row += STORE_THREADS) {
+    const TileRow r = tile_row(p, m_tile, row);
+    rowoff[row] = r.valid ? out_row_off(p, r) : -1;
+  }
+  asm volatile("bar.sync 2, %0;" ::"n"(STORE_THREADS) : "memory");
+  const bool geglu = (p.act == PFD_ACT_GEGLU);
+  const int cpr = (geglu ? BN / 2 : BN) / 8;          // 16-byte chunks per tile row
+  const int col_base = n_tile * cpr * 8;
+  const int n_out = geglu ? p.N / 2 : p.N;
+  const bool add_res = p.residual && !geglu;
+  const int total = BM * cpr;
+  long long off[STORE_BATCH];
+  int soff[STORE_BATCH];
+  uint4 res[STORE_BATCH];
+  auto load_batch = [&](int i0) {
+#pragma unroll
+    for (int b = 0; b < STORE_BATCH; ++b) {
+      const int idx = i0 + b * STORE_THREADS;
+      off[b] = -1;
+      if (idx < total) {
+        const int row = idx / cpr, ch = idx - row * cpr;
+        const int col = col_base + 8 * ch;
+        const long long ro = rowoff[row];
+        soff[b] = row * C_PITCH + ch * 16;
+        if (ro >= 0 && col < n_out) {
+          off[b] = ro + out_col_off(p, col);
+          if (add_res) res[b] = __ldg(reinterpret_cast<const uint4*>(p.residual + off[b]));
+        }
+      }
+    }
+  };
+  load_batch(t);
+  mbar_wait(c_full, parity);
+#pragma unroll 1
+  for (int i0 = t; i0 < total; i0 += STORE_THREADS * STORE_BATCH) {
+#pragma unroll
+    for (int b = 0; b < STORE_BATCH; ++b) {
+      if (off[b] < 0) continue;
+      uint4 v = *reinterpret_cast<const uint4*>(cbuf + soff[b]);
+      if (add_res) {
+        __half2* h = reinterpret_cast<__half2*>(&v);
+        const __half2* r = reinterpret_cast<const __half2*>(&res[b]);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) h[k] = __hadd2(h[k], r[k]);
+      }
+      *reinterpret_cast<uint4*>(p.out + off[b]) = v;
+    }
+    if (i0 + STORE_THREADS * STORE_BATCH < total) load_batch(i0 + STORE_THREADS * STORE_BATCH);
+  }
+}
+
+// Direct epilogue from the accumulator registers, for the tiles the staged epilogue does not take:
 //   * split-K slice: raw fp32 partials -> workspace (bias etc. in splitk_finish_kernel);
-//   * GEGLU (tile packed [value(BN/2) | gate(BN/2)], pack_geglu): out = fp16(value) * fp16(gelu(fp16(gate)));
-//   * otherwise fp16(act(acc * alpha + bias + row add)), then the residual added in fp16 - the reference's
-//     `x + f(h)` on fp16 tensors - or, for element-strided outputs (V^T), in fp32 before the single rounding.
+//   * element-strided outputs (V^T, !vec_ok): as gemm_stage_tile, but the residual is added in fp32 before the
+//     single rounding.
 template <int BN>
 __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const float (&acc)[BN / 2], int cw, int tile,
                                               int split, int m_tiles) {
   const int wl = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const int n_tile = tile % p.n_tiles;
   const int m_tile = tile / p.n_tiles;
-  const int tx = m_tile % p.tiles_w;
-  const int ty = (m_tile / p.tiles_w) % p.tiles_h;
-  const int tn = m_tile / (p.tiles_w * p.tiles_h);
   const bool geglu = (p.act == PFD_ACT_GEGLU);
   const int n_out = geglu ? p.N / 2 : p.N;
   const int col_base = n_tile * (geglu ? BN / 2 : BN);
   const int cq = 2 * (lane & 3);
-  const bool plain_cols = p.cdiv >= p.N;
   int rows[2];
   bool valid[2];
   long long row_off[2];
@@ -289,36 +488,21 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const float (
   for (int i = 0; i < 2; ++i) {
     const int row = cw * 64 + wl * 16 + (lane >> 2) + 8 * i;
     rows[i] = row;
-    const int x = tx * p.bw + row % p.bw;
-    const int y = ty * p.bh + (row / p.bw) % p.bh;
-    const int n = tn * p.bn + row / (p.bw * p.bh);
-    valid[i] = (x < p.W) && (y < p.H) && (n < p.NB);
-    row_off[i] = (long long)(n / p.ndiv) * p.so_n1 + (long long)(n % p.ndiv) * p.so_n0 + (long long)y * p.so_y +
-                 (long long)x * p.so_x;
-    rowadd_row[i] = (p.rowadd && valid[i]) ? p.rowadd + (long long)n * p.rowadd_ld : nullptr;
+    const TileRow r = tile_row(p, m_tile, row);
+    valid[i] = r.valid;
+    row_off[i] = out_row_off(p, r);
+    rowadd_row[i] = (p.rowadd && valid[i]) ? p.rowadd + (long long)r.n * p.rowadd_ld : nullptr;
   }
-  auto coff_of = [&](int c) -> long long {
-    return plain_cols ? (long long)c * p.so_c0 : (long long)(c / p.cdiv) * p.so_c1 + (long long)(c % p.cdiv) * p.so_c0;
-  };
   // fp16 pair (lo, hi) -> output columns c, c + 1 of row i
   auto store2 = [&](int i, int c, float lo, float hi) {
-    const long long o0 = row_off[i] + coff_of(c);
-    if (p.vec_ok) {
-      __half2 h = __floats2half2_rn(lo, hi);
-      if (p.residual) {
-        const uint32_t r = ldg_h2(p.residual + o0);
-        h = __hadd2(h, *reinterpret_cast<const __half2*>(&r));
-      }
-      *reinterpret_cast<__half2*>(p.out + o0) = h;
-    } else {
-      const long long o1 = row_off[i] + coff_of(c + 1);
-      if (p.residual) {
-        lo += __half2float(p.residual[o0]);
-        hi += __half2float(p.residual[o1]);
-      }
-      p.out[o0] = __float2half_rn(lo);
-      p.out[o1] = __float2half_rn(hi);
+    const long long o0 = row_off[i] + out_col_off(p, c);
+    const long long o1 = row_off[i] + out_col_off(p, c + 1);
+    if (p.residual) {
+      lo += __half2float(p.residual[o0]);
+      hi += __half2float(p.residual[o1]);
     }
+    p.out[o0] = __float2half_rn(lo);
+    p.out[o1] = __float2half_rn(hi);
   };
 
   if (p.splits > 1) {
@@ -356,9 +540,7 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const float (
         const float2 gf = __half22float2(__floats2half2_rn(fmaf(g[0], alpha, bg0), fmaf(g[1], alpha, bg1)));
         const __half2 o = __hmul2(a, __floats2half2_rn(gelu_sig(gf.x), gelu_sig(gf.y)));
         const float2 of = __half22float2(o);
-        const long long o0 = row_off[i] + coff_of(col);
-        if (p.vec_ok) *reinterpret_cast<__half2*>(p.out + o0) = o;
-        else store2(i, col, of.x, of.y);
+        store2(i, col, of.x, of.y);
       }
     }
     return;
@@ -406,12 +588,18 @@ gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
   const uint32_t base = (raw_addr + 1023u) & ~1023u;
   const uint32_t smemA = base;                                        // [STAGES][A tile]
   const uint32_t smemB = base + STAGES * STAGE_A_BYTES;               // [STAGES][B tile]
-  const uint32_t bars = base + STAGES * Cfg::STAGE_BYTES;
-  // barrier layout: full[STAGES] | empty[STAGES]
+  const uint32_t cbuf_off = base - raw_addr + STAGES * Cfg::STAGE_BYTES;
+  uint8_t* const cbuf = smem_raw + cbuf_off;                          // staged output tile [BM][C_PITCH]
+  long long* const rowoff = reinterpret_cast<long long*>(cbuf + BM * Cfg::C_PITCH);   // [2][BM]
+  const uint32_t bars = base + STAGES * Cfg::STAGE_BYTES + Cfg::C_BYTES;
+  // barrier layout: full[STAGES] | empty[STAGES] | c_full | c_empty
   auto full_bar = [&](int s) { return bars + 8u * s; };
   auto empty_bar = [&](int s) { return bars + 8u * (STAGES + s); };
+  const uint32_t c_full = bars + 16u * STAGES, c_empty = c_full + 8u;
 
   const int wg = threadIdx.x >> 7;
+  // staged epilogue for every tile of the launch except stream-K contributors (see gemm_stage_tile)
+  const bool staged = p.vec_ok && p.splits == 1;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.nseg; ++s) tma_prefetch_desc(&p.tmA[s]);
@@ -420,6 +608,8 @@ gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
       mbar_init(full_bar(s), 1);
       mbar_init(empty_bar(s), 8);           // one arrival per consumer warp
     }
+    mbar_init(c_full, 8);                   // one arrival per consumer warp
+    mbar_init(c_empty, STORE_THREADS / 32); // one arrival per store warp
     mbar_fence_init();
   }
   __syncthreads();
@@ -431,9 +621,19 @@ gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
   const int total_tiles = m_tiles * p.n_tiles;
 
   if (wg == 0) {
-    // ------------------------------------------------------------ TMA producer (one thread)
-    setmaxnreg_dec<40>();
-    if (threadIdx.x == 0) {
+    // ------------------------------------------------------------ TMA producer (thread 0) + store warps (warps 1-3)
+    setmaxnreg_dec<Cfg::PRODUCER_REGS>();
+    if (threadIdx.x >= 32 && staged) {
+      uint32_t c_phase = 0;
+      WorkItem w;
+      for (int wi = 0; gemm_work<SK>(p, wi, total_tiles, w); ++wi) {
+        if (SK && w.mode == 1) continue;
+        gemm_store_tile<BN>(p, w.tile, cbuf, rowoff + (c_phase ? BM : 0), c_full, c_phase);
+        __syncwarp();
+        if ((threadIdx.x & 31) == 0) mbar_arrive(c_empty);
+        c_phase ^= 1u;
+      }
+    } else if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       WorkItem w;
@@ -474,11 +674,11 @@ gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
     }
   } else {
     // ------------------------------------------------------------ wgmma consumers (64 rows each) + epilogue
-    setmaxnreg_inc<232>();
+    setmaxnreg_inc<Cfg::CONSUMER_REGS>();
     const int cw = wg - 1;
     const bool arrive_lane = (threadIdx.x & 31) == 0;
     int stage = 0;
-    uint32_t phase = 0;
+    uint32_t phase = 0, c_phase = 0;
     float acc[BN / 2];
     WorkItem w;
     for (int wi = 0; gemm_work<SK>(p, wi, total_tiles, w); ++wi) {
@@ -509,7 +709,15 @@ gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
         continue;
       }
       if (SK && w.mode == 2) sk_gather<BN>(p, acc, w.tile - p.sk_dp_tiles);
-      gemm_epilogue<BN>(p, acc, cw, w.tile, w.slot, m_tiles);
+      if (staged) {
+        mbar_wait(c_empty, c_phase ^ 1u);   // the store warps have read the previous tile out of the buffer
+        gemm_stage_tile<BN>(p, acc, cw, w.tile, cbuf);
+        __syncwarp();
+        if (arrive_lane) mbar_arrive(c_full);
+        c_phase ^= 1u;
+      } else {
+        gemm_epilogue<BN>(p, acc, cw, w.tile, w.slot, m_tiles);
+      }
     }
   }
 }
