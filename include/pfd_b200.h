@@ -250,6 +250,33 @@ PFD_API int pfd_canny_f32(const void* x, int32_t src_is_f32, int32_t B, int32_t 
 /* ToTensor(ToPILImage(x)) = floor(x*255)/255 as float32 (controlnet.py:345-348, preprocess type 'input'). */
 PFD_API int pfd_image_u8_roundtrip_f32(const void* x, int32_t src_is_f32, int64_t n, float* out, void* stream);
 
+/*
+ * ControlNet.preprocess(type='hed' / 'softedge_v11p') (controlnet.py:370-376 -> controlnet_annotator/hed/__init__.py:
+ * 102-128): the glue around the 13 convolutions of ControlNetHED_Apache2 (hed/__init__.py:23-59), which run on
+ * pfd_gemm_f16.  The network runs at an activation scale s: the input and every conv bias are multiplied by s, so each
+ * activation and side map is s times the reference's (ReLU convs and max-pool are positively homogeneous).
+ *
+ * pfd_hed_input_f16: NCHW [B,3,H,W] image in [0,1] (fp16 or fp32) -> channel-last fp16 [B,H,W,Cpad],
+ *   out = (u8 - norm[c]) * scale with u8 = x.mul(255).byte() (ToPILImage, rounded in x's dtype) and the
+ *   `x - self.norm` of hed/__init__.py:52; channels 3..Cpad-1 are zero.  norm: device float[3].
+ * pfd_hed_pool_side_f16: one read of a block output x [B,h,w,C] fp16 (C % 8 == 0, 16-byte aligned) writes
+ *   side [B,h,w] fp32 = x . proj_w + *proj_b (the block's 1x1 projection, hed/__init__.py:38; fp32 accumulation) and,
+ *   when pooled != NULL, pooled [B,h/2,w/2,C] fp16 = 2x2 stride-2 max-pool, floor for odd h / w (F.max_pool2d,
+ *   hed/__init__.py:34).  proj_w: device float[C]; proj_b: device float[1].
+ * pfd_hed_fuse_f32: apply_hed after the network (hed/__init__.py:119-127) for nsides <= PFD_HED_MAX_SIDES fp32 side
+ *   maps [B,h_k,w_k] (host array of device pointers and sizes): cv2.resize(INTER_LINEAR) of each to H x W, times
+ *   inv_scale, np.mean over the maps (sequential float32 sum / n), sigmoid in float64, trunc(clip(edge*255, 0, 255)),
+ *   then /255 (ToTensor) -> float32 [B,3,H,W] with three equal channels.
+ * All three are asynchronous on `stream` and graph-capturable.
+ */
+#define PFD_HED_MAX_SIDES 5
+PFD_API int pfd_hed_input_f16(const void* x, int32_t src_is_f32, int32_t B, int32_t H, int32_t W, int32_t Cpad,
+                              const float* norm, float scale, void* out, void* stream);
+PFD_API int pfd_hed_pool_side_f16(const void* x, int32_t B, int32_t h, int32_t w, int32_t C, const float* proj_w,
+                                  const float* proj_b, float* side, void* pooled, void* stream);
+PFD_API int pfd_hed_fuse_f32(const float* const* sides, const int32_t* side_h, const int32_t* side_w, int32_t nsides,
+                             int32_t B, int32_t H, int32_t W, float inv_scale, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

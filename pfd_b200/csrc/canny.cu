@@ -26,20 +26,7 @@ __device__ __forceinline__ void pdl_enter_c() {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
 
-// ToPILImage on a float tensor: pic.mul(255).byte() - the product is rounded in the tensor's dtype, then truncated
-template <typename T>
-__device__ __forceinline__ uint32_t to_u8(T v);
-template <>
-__device__ __forceinline__ uint32_t to_u8<float>(float v) {
-  const float m = v * 255.f;
-  return (uint32_t)(unsigned char)(int)m;
-}
-template <>
-__device__ __forceinline__ uint32_t to_u8<__half>(__half v) {
-  const float m = __half2float(__hmul(v, __float2half_rn(255.f)));
-  return (uint32_t)(unsigned char)(int)m;
-}
-
+// to_u8<T> (common.h): ToPILImage's x.mul(255).byte()
 template <typename T>
 __global__ void canny_pack_kernel(const T* __restrict__ x, int B, int H, int W, uint32_t* __restrict__ rgbx) {
   pdl_enter_c();

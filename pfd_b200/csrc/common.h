@@ -1,5 +1,6 @@
 // Host-side shared helpers for the C-ABI translation units (error text, launch counter).
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -54,6 +55,23 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
   cfg.numAttrs = use_pdl() ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
+
+#ifdef __CUDACC__
+// ToPILImage on a float tensor: pic.mul(255).byte() - the product is rounded in the tensor's dtype, then truncated
+// (torchvision ToPILImage, controlnet.py:339; shared by the Canny and HED annotators)
+template <typename T>
+__device__ __forceinline__ uint32_t to_u8(T v);
+template <>
+__device__ __forceinline__ uint32_t to_u8<float>(float v) {
+  const float m = v * 255.f;
+  return (uint32_t)(unsigned char)(int)m;
+}
+template <>
+__device__ __forceinline__ uint32_t to_u8<__half>(__half v) {
+  const float m = __half2float(__hmul(v, __float2half_rn(255.f)));
+  return (uint32_t)(unsigned char)(int)m;
+}
+#endif
 
 inline int num_sms() {
   static int n = 0;

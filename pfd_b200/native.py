@@ -30,7 +30,9 @@ EXPORTS = [
     "pfd_patch_merge_gather_f16", "pfd_patchify_f16", "pfd_flash_attn_f16",
     "pfd_flash_attn_strided_f16", "pfd_ddim_begin_step", "pfd_vae_posterior_f16",
     "pfd_canny_workspace_bytes", "pfd_canny_f32", "pfd_image_u8_roundtrip_f32",
+    "pfd_hed_input_f16", "pfd_hed_pool_side_f16", "pfd_hed_fuse_f32",
 ]
+PFD_HED_MAX_SIDES = 5
 
 
 class GemmDesc(ctypes.Structure):
@@ -125,6 +127,12 @@ def load() -> ctypes.CDLL:
     lib.pfd_canny_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p,
                                   POINTER(c_int32), c_void_p]
     lib.pfd_image_u8_roundtrip_f32.argtypes = [c_void_p, c_int32, c_int64, c_void_p, c_void_p]
+    lib.pfd_hed_input_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_float,
+                                      c_void_p, c_void_p]
+    lib.pfd_hed_pool_side_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p,
+                                          c_void_p, c_void_p]
+    lib.pfd_hed_fuse_f32.argtypes = [POINTER(c_void_p), POINTER(c_int32), POINTER(c_int32), c_int32, c_int32, c_int32,
+                                     c_int32, c_float, c_void_p, c_void_p]
     for name in EXPORTS:
         if hasattr(lib, name) and name not in ("pfd_version", "pfd_last_error", "pfd_launch_count",
                                                "pfd_canny_workspace_bytes"):
@@ -499,6 +507,61 @@ def image_u8_roundtrip(x: torch.Tensor) -> torch.Tensor:
     out = torch.empty(x.shape, device=x.device, dtype=torch.float32)
     _check(load().pfd_image_u8_roundtrip_f32(x.data_ptr(), int(x.dtype == torch.float32), x.numel(), out.data_ptr(),
                                              stream_ptr()), "pfd_image_u8_roundtrip_f32")
+    return out
+
+
+def _chk32(t: torch.Tensor, name: str) -> None:
+    if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
+        raise RuntimeError(f"{name}: expected a contiguous CUDA fp32 tensor, got {t.dtype} on {t.device}")
+
+
+def hed_input(x: torch.Tensor, norm: torch.Tensor, scale: float, cpad: int = 3) -> torch.Tensor:
+    """NCHW [B,3,H,W] image in [0,1] (fp16/fp32) -> channel-last fp16 [B,H,W,cpad] = (x.mul(255).byte() - norm) * scale,
+    zero pad channels (pfd_hed_input_f16).  norm: CUDA fp32 [3]."""
+    if x.dim() != 4 or x.shape[1] != 3 or not x.is_cuda or x.dtype not in (torch.float16, torch.float32):
+        raise RuntimeError(f"hed_input: expected a CUDA fp16/fp32 [B,3,H,W] image, got {tuple(x.shape)} {x.dtype}")
+    _chk32(norm, "hed_input norm")
+    x = x.contiguous()
+    B, _, H, W = x.shape
+    out = torch.empty((B, H, W, cpad), device=x.device, dtype=torch.float16)
+    _check(load().pfd_hed_input_f16(x.data_ptr(), int(x.dtype == torch.float32), B, H, W, cpad, norm.data_ptr(),
+                                    float(scale), out.data_ptr(), stream_ptr()), "pfd_hed_input_f16")
+    return out
+
+
+def hed_pool_side(x: torch.Tensor, proj_w: torch.Tensor, proj_b: torch.Tensor, pool: bool = True):
+    """Block output x [B,h,w,C] fp16 -> (side [B,h,w] fp32 = x . proj_w + proj_b, 2x2 max-pooled [B,h/2,w/2,C] fp16 or
+    None), both from one read of x (pfd_hed_pool_side_f16).  proj_w: CUDA fp32 [C]; proj_b: CUDA fp32 [1]."""
+    _chk16(x, "hed_pool_side x")
+    _chk32(proj_w, "hed_pool_side proj_w")
+    _chk32(proj_b, "hed_pool_side proj_b")
+    x = x.contiguous()
+    B, h, w, C = x.shape
+    if proj_w.numel() != C:
+        raise RuntimeError(f"hed_pool_side: proj_w has {proj_w.numel()} entries for C={C}")
+    side = torch.empty((B, h, w), device=x.device, dtype=torch.float32)
+    pooled = torch.empty((B, h // 2, w // 2, C), device=x.device, dtype=torch.float16) if pool else None
+    _check(load().pfd_hed_pool_side_f16(x.data_ptr(), B, h, w, C, proj_w.data_ptr(), proj_b.data_ptr(),
+                                        side.data_ptr(), _p(pooled), stream_ptr()), "pfd_hed_pool_side_f16")
+    return side, pooled
+
+
+def hed_fuse(sides: Sequence[torch.Tensor], H: int, W: int, inv_scale: float = 1.0) -> torch.Tensor:
+    """apply_hed after the network: fp32 side maps [B,h_k,w_k] -> float32 [B,3,H,W] (pfd_hed_fuse_f32)."""
+    n = len(sides)
+    if not 1 <= n <= PFD_HED_MAX_SIDES:
+        raise RuntimeError(f"hed_fuse: {n} side maps (1..{PFD_HED_MAX_SIDES})")
+    B = sides[0].shape[0]
+    for s in sides:
+        _chk32(s, "hed_fuse side map")
+        if s.dim() != 3 or s.shape[0] != B:
+            raise RuntimeError(f"hed_fuse: side maps must be [B,h,w] with B={B}, got {tuple(s.shape)}")
+    out = torch.empty((B, 3, H, W), device=sides[0].device, dtype=torch.float32)
+    ptrs = (c_void_p * n)(*[s.data_ptr() for s in sides])
+    hs = (c_int32 * n)(*[s.shape[1] for s in sides])
+    ws = (c_int32 * n)(*[s.shape[2] for s in sides])
+    _check(load().pfd_hed_fuse_f32(ptrs, hs, ws, n, B, H, W, float(inv_scale), out.data_ptr(), stream_ptr()),
+           "pfd_hed_fuse_f32")
     return out
 
 
