@@ -141,6 +141,10 @@ PFD_API int pfd_softmax_f16(void* s, int64_t batch, int32_t rows, int32_t cols, 
 /* sinusoidal timestep embedding [cos | sin], fp32 math, fp16 out (diffusion_utils.py:131-151). */
 PFD_API int pfd_timestep_embedding_f16(const int64_t* t, int32_t n, int32_t dim, float max_period,
                                void* out, void* stream);
+/* the same embedding for float32 (fractional) timesteps t[n], as the k-diffusion samplers evaluate the UNet at
+ * t(sigma) (diffusion_utils.py:131-146 accepts any float t); equals pfd_timestep_embedding_f16 at integer t. */
+PFD_API int pfd_timestep_embedding_ft_f16(const float* t, int32_t n, int32_t dim, float max_period, void* out,
+                                          void* stream);
 
 /* nearest-neighbour 2x upsample, channel-last (openaimodel.py:114, autokl_modules.py:54). */
 PFD_API int pfd_upsample2x_f16(const void* x, int32_t NB, int32_t H, int32_t W, int32_t C, void* out,
@@ -194,6 +198,29 @@ PFD_API int pfd_vae_posterior_f16(const void* moments, int32_t B, int32_t zc, in
 /* Device-side loop header of one DDIM step (ddim.py:108-113): *step -= 1; t_out[0..nb) = ttab[*step].
  * Lets one CUDA graph hold several (or all) steps of the sampling loop with no host work in between. */
 PFD_API int pfd_ddim_begin_step(int32_t* step, const int64_t* ttab, int64_t* t_out, int32_t nb, void* stream);
+
+/*
+ * k-diffusion samplers: Euler ancestral and DPM-Solver++(2M) (sampler.py:19-27,84-104, whose `sample` (:56-82) never
+ * wraps the eps-prediction UNet as a denoiser nor applies CFG).  Every step of either type is one affine update with a
+ * host-computed row coef[step*PFD_KSAMPLER_NCOEF + {0..5}] = {sigma, a, b, c, u, c_in_next} (fp32):
+ *   e  = e_u + guidance*(e_c - e_u)   (cfg != 0: eps = [uncond | cond] halves of half_n fp16 elements)
+ *      = guidance*eps                 (cfg == 0: one half, as the DDIM sampler's e_t = eps * scale)
+ *   D  = x - sigma*e                  (the denoised estimate; x is the fp32 state, UNet input x*c_in)
+ *   x' = a*x + b*D + c*d_prev + u*noise   (noise: fp16, NULL = none; u = sigma_up of an ancestral step)
+ * The call then stores x' to x, D to d_prev, and fp16(x'*c_in_next) to unet_in (both halves when cfg != 0), i.e. the
+ * next step's UNet input; on step == last_step also fp16(x') to out [half_n].  log_tab (optional): int32 slot per step
+ * (-1 = none); the step's fp16 UNet input and D are also stored at log_xt / log_x0 + slot*half_n.
+ * The step index is read from the device int *step, so a captured CUDA graph can be replayed for every step.
+ */
+#define PFD_KSAMPLER_NCOEF 6
+PFD_API int pfd_ksampler_step_f32(const void* eps, int32_t cfg, float guidance, int64_t half_n, const float* coef,
+                                  const int32_t* step, int32_t last_step, float* x, float* d_prev, const void* noise,
+                                  void* unet_in, void* out, const int32_t* log_tab, void* log_xt, void* log_x0,
+                                  void* stream);
+/* Device-side loop header of one k-sampler step: *step += 1 (clamped to [0, nsteps)); t_out[0..nb) = ttab[*step], the
+ * step's float timestep t(sigma).  Starts from *step = -1. */
+PFD_API int pfd_ksampler_begin_step(int32_t* step, const float* ttab, int32_t nsteps, float* t_out, int32_t nb,
+                                    void* stream);
 
 /* Swin window plumbing on channel-last [B,H,W,C] (swin.py:269-304): pad + cyclic shift + window
  * partition in one gather (fwd) and the inverse scatter + crop (bwd). */

@@ -1,7 +1,7 @@
 """pfd_b200 — H100-native (sm_90a) implementation of the Prompt-Free-Diffusion inference hot path.
 
 Public surface (mirrors the reference's lib.model_zoo / lib.cfg_helper plugin API):
-    from pfd_b200 import get_model, register, model_cfg_bank, DDIMSampler
+    from pfd_b200 import get_model, register, model_cfg_bank, DDIMSampler, Sampler
     net = get_model()(model_cfg_bank()('pfd_seecoder_with_controlnet')); net.to('cuda')
     c = net.ctx_encode(img, 'image'); x, _ = DDIMSampler(net).sample(...); im = net.vae_decode(x, 'image')
 All arithmetic runs in the hand-written CUDA kernels behind include/pfd_b200.h (pfd_b200/native.py);
@@ -15,4 +15,7 @@ def __getattr__(name):
     if name == "DDIMSampler":
         from .ddim import DDIMSampler
         return DDIMSampler
+    if name == "Sampler":
+        from .sampler import Sampler
+        return Sampler
     raise AttributeError(name)

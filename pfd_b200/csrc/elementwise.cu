@@ -338,7 +338,10 @@ softmax_rows_kernel(__half* __restrict__ s, long long batch, int rows, int cols,
 }
 
 // ------------------------------------------------------------------------------------ misc
-__global__ void timestep_embedding_kernel(const long long* __restrict__ t, int n, int dim,
+// T = long long (integer DDIM timesteps) or float (fractional k-sampler timesteps); (float)t is exact for t <= 2^24,
+// so both agree bit for bit at integer t
+template <typename T>
+__global__ void timestep_embedding_kernel(const T* __restrict__ t, int n, int dim,
                                           float max_period, __half* __restrict__ out) {
   pdl_enter();
   const int half_d = dim / 2;
@@ -741,9 +744,18 @@ extern "C" PFD_API int pfd_softmax_f16(void* s, int64_t batch, int32_t rows, int
 extern "C" PFD_API int pfd_timestep_embedding_f16(const int64_t* t, int32_t n, int32_t dim, float max_period,
                                           void* out, void* stream) {
   const int total = n * (dim / 2);
-  launch_k(timestep_embedding_kernel, dim3((total + 127) / 128), dim3(128), (size_t)(0), static_cast<cudaStream_t>(stream), 
+  launch_k(timestep_embedding_kernel<long long>, dim3((total + 127) / 128), dim3(128), (size_t)(0), static_cast<cudaStream_t>(stream),
       reinterpret_cast<const long long*>(t), n, dim, max_period, static_cast<__half*>(out));
   return check_launch("timestep_embedding");
+}
+
+extern "C" PFD_API int pfd_timestep_embedding_ft_f16(const float* t, int32_t n, int32_t dim, float max_period,
+                                                     void* out, void* stream) {
+  if (!t || !out || n <= 0 || dim <= 0) return set_error("pfd_timestep_embedding_ft_f16: null/empty argument");
+  const int total = n * (dim / 2);
+  launch_k(timestep_embedding_kernel<float>, dim3((total + 127) / 128), dim3(128), (size_t)(0),
+           static_cast<cudaStream_t>(stream), t, n, dim, max_period, static_cast<__half*>(out));
+  return check_launch("timestep_embedding_ft");
 }
 
 extern "C" PFD_API int pfd_upsample2x_f16(const void* x, int32_t NB, int32_t H, int32_t W, int32_t C, void* out,

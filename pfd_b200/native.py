@@ -31,7 +31,9 @@ EXPORTS = [
     "pfd_flash_attn_strided_f16", "pfd_ddim_begin_step", "pfd_vae_posterior_f16",
     "pfd_canny_workspace_bytes", "pfd_canny_f32", "pfd_image_u8_roundtrip_f32",
     "pfd_hed_input_f16", "pfd_hed_pool_side_f16", "pfd_hed_fuse_f32",
+    "pfd_timestep_embedding_ft_f16", "pfd_ksampler_step_f32", "pfd_ksampler_begin_step",
 ]
+PFD_KSAMPLER_NCOEF = 6
 PFD_HED_MAX_SIDES = 5
 
 
@@ -93,6 +95,7 @@ def load() -> ctypes.CDLL:
     lib.pfd_softmax_f16.argtypes = [c_void_p, c_int64, c_int32, c_int32, c_int64, c_float, c_void_p,
                                     c_int32, c_void_p, c_int32, c_void_p]
     lib.pfd_timestep_embedding_f16.argtypes = [c_void_p, c_int32, c_int32, c_float, c_void_p, c_void_p]
+    lib.pfd_timestep_embedding_ft_f16.argtypes = [c_void_p, c_int32, c_int32, c_float, c_void_p, c_void_p]
     lib.pfd_upsample2x_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]
     lib.pfd_nchw_to_nhwc_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
                                          c_float, c_float, c_void_p, c_void_p]
@@ -122,6 +125,10 @@ def load() -> ctypes.CDLL:
                                                c_int32, c_int32, POINTER(c_int64), POINTER(c_int64),
                                                POINTER(c_int64), c_float, c_int64, c_int64, c_void_p]
     lib.pfd_ddim_begin_step.argtypes = [c_void_p, c_void_p, c_void_p, c_int32, c_void_p]
+    lib.pfd_ksampler_step_f32.argtypes = [c_void_p, c_int32, c_float, c_int64, c_void_p, c_void_p, c_int32, c_void_p,
+                                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                          c_void_p]
+    lib.pfd_ksampler_begin_step.argtypes = [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_void_p]
     lib.pfd_canny_workspace_bytes.argtypes = [c_int32, c_int32, c_int32]
     lib.pfd_canny_workspace_bytes.restype = c_int64
     lib.pfd_canny_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p,
@@ -383,9 +390,16 @@ def softmax_(s: torch.Tensor, scale: float, *, bias: Optional[torch.Tensor] = No
 
 
 def timestep_embedding(t: torch.Tensor, dim: int, max_period: float = 10000.0) -> torch.Tensor:
+    """[cos | sin] embedding of int64 timesteps (the DDIM sampler) or float32 fractional ones (the k-samplers)."""
     out = torch.empty((t.shape[0], dim), device=t.device, dtype=torch.float16)
-    _check(load().pfd_timestep_embedding_f16(t.data_ptr(), t.shape[0], dim, max_period, out.data_ptr(),
-                                             stream_ptr()), "pfd_timestep_embedding_f16")
+    if t.dtype == torch.int64:
+        _check(load().pfd_timestep_embedding_f16(t.data_ptr(), t.shape[0], dim, max_period, out.data_ptr(),
+                                                 stream_ptr()), "pfd_timestep_embedding_f16")
+    elif t.dtype == torch.float32:
+        _check(load().pfd_timestep_embedding_ft_f16(t.contiguous().data_ptr(), t.shape[0], dim, max_period,
+                                                    out.data_ptr(), stream_ptr()), "pfd_timestep_embedding_ft_f16")
+    else:
+        raise RuntimeError(f"timestep_embedding: int64 or float32 timesteps expected, got {t.dtype}")
     return out
 
 
@@ -469,6 +483,40 @@ def ddim_begin_step(step: torch.Tensor, ttab: torch.Tensor, t_out: torch.Tensor)
         raise RuntimeError("ddim_begin_step: step int32, ttab / t_out int64 expected")
     _check(load().pfd_ddim_begin_step(step.data_ptr(), ttab.data_ptr(), t_out.data_ptr(), t_out.numel(),
                                       stream_ptr()), "pfd_ddim_begin_step")
+
+
+def ksampler_step(eps: torch.Tensor, cfg: bool, guidance: float, coef: torch.Tensor, step: torch.Tensor,
+                  last_step: int, x: torch.Tensor, d_prev: torch.Tensor, unet_in: torch.Tensor, out: torch.Tensor, *,
+                  noise: Optional[torch.Tensor] = None, log_tab: Optional[torch.Tensor] = None,
+                  log_xt: Optional[torch.Tensor] = None, log_x0: Optional[torch.Tensor] = None) -> None:
+    """One k-sampler step (see pfd_ksampler_step_f32): CFG combine, D = x - sigma*e, x = a*x + b*D + c*d_prev + u*noise,
+    d_prev = D, unet_in = fp16(x*c_in_next) (both CFG halves), out = fp16(x) on the last step."""
+    half_n = x.numel()
+    _chk16(eps, "ksampler_step eps")
+    for t, name in ((x, "x"), (d_prev, "d_prev"), (coef, "coef")):
+        _chk32(t, f"ksampler_step {name}")
+    if step.dtype != torch.int32 or coef.dim() != 2 or coef.shape[1] != PFD_KSAMPLER_NCOEF:
+        raise RuntimeError("ksampler_step: int32 step and a [steps, 6] coefficient table expected")
+    halves = 2 if cfg else 1
+    if eps.numel() != halves * half_n or unet_in.numel() != halves * half_n or out.numel() != half_n \
+            or d_prev.numel() != half_n or (noise is not None and noise.numel() != half_n):
+        raise RuntimeError("ksampler_step: eps / unet_in / out / d_prev / noise sizes do not match the state")
+    _chk16(unet_in, "ksampler_step unet_in")
+    _chk16(out, "ksampler_step out")
+    if noise is not None:
+        _chk16(noise, "ksampler_step noise")
+    _check(load().pfd_ksampler_step_f32(eps.data_ptr(), int(cfg), float(guidance), half_n, coef.data_ptr(),
+                                        step.data_ptr(), int(last_step), x.data_ptr(), d_prev.data_ptr(), _p(noise),
+                                        unet_in.data_ptr(), out.data_ptr(), _p(log_tab), _p(log_xt), _p(log_x0),
+                                        stream_ptr()), "pfd_ksampler_step_f32")
+
+
+def ksampler_begin_step(step: torch.Tensor, ttab: torch.Tensor, t_out: torch.Tensor) -> None:
+    """Device-side loop header: step += 1; t_out[:] = ttab[step] (see pfd_ksampler_begin_step)."""
+    if step.dtype != torch.int32 or ttab.dtype != torch.float32 or t_out.dtype != torch.float32:
+        raise RuntimeError("ksampler_begin_step: step int32, ttab / t_out float32 expected")
+    _check(load().pfd_ksampler_begin_step(step.data_ptr(), ttab.data_ptr(), ttab.numel(), t_out.data_ptr(),
+                                          t_out.numel(), stream_ptr()), "pfd_ksampler_begin_step")
 
 
 def vae_posterior(moments: torch.Tensor, zc: int, *, noise: Optional[torch.Tensor] = None, scale: float = 1.0,
