@@ -47,9 +47,21 @@ PFD_API const char* pfd_last_error(void);
 PFD_API int64_t pfd_launch_count(void);
 /* Run-time tuning switches, so that variants can be A/B-timed inside one process (tools/ab_unet.py); name == NULL
  * resets all of them to the built-in defaults.  Unknown names are stored and ignored.  Known names (default):
- *   gemm_streamk (0)   stream-K tail of the persistent GEMM
+ *   gemm_streamk (0)   stream-K tail of the persistent GEMM (ignored in deterministic mode)
  *   flash_poly_mod (0) exponent path of the attention softmax for d <= 64: 1 = packed-half MUFU, n > 1 = every n-th
- *                      pair on the FMA pipe */
+ *                      pair on the FMA pipe
+ *   deterministic (0)  1 = deterministic mode: with the same build on the same GPU architecture, every output of the
+ *                      library is a bitwise function of the sample's own inputs - the same across runs and processes,
+ *                      batch compositions (sample i of a batch equals the sample computed alone), GPU counts and SM
+ *                      counts.  GroupNorm adds its statistics in a fixed order (no float atomics; chunks sized from
+ *                      HW and C only), and the GEMM never splits K and ignores gemm_streamk.  Results stay within
+ *                      rounding of the default mode but are not bit-equal to it.  The default is 1 when the
+ *                      environment variable PFD_DETERMINISTIC=1 is set when the library is loaded; a reset
+ *                      (name == NULL) returns to that default.  CUDA graphs captured before the switch keep the
+ *                      mode they were captured in: the Python package's set_deterministic() also drops its cached
+ *                      graphs, setting this option directly does not.
+ *   plan_sms (0)       test only: SM count the GEMM and GroupNorm plan their grids and split-K with; 0 = the
+ *                      device's, otherwise min(value, the device's). */
 PFD_API int pfd_set_option(const char* name, int32_t value);
 
 /*
@@ -118,6 +130,10 @@ PFD_API int pfd_gemm_f16(const pfd_gemm_desc* d);
  *     32-bit arrival counter per image for the single-pass kernel),
  *     16-byte aligned.  zero_ws != 0: the call zeroes it first (one extra memset node); zero_ws == 0: the
  *     caller guarantees it is already zero (e.g. one bulk memset of many slots per network evaluation).
+ * Deterministic mode (pfd_set_option "deterministic"): each CTA's statistics are combined in a fixed order into one
+ *     fp64 partial per (image, group, pixel chunk) in a library-owned per-device buffer, and the last CTA of each
+ *     image adds them in chunk order and overwrites ws (which then need not be zero).  Limits: NB <= 64, C <= 6144.
+ *     The first deterministic call on a device allocates that buffer and must not be inside a stream capture.
  */
 PFD_API int pfd_groupnorm_f16(const void* x1, int32_t c1, const void* x2, int32_t c2, int32_t NB,
                       int64_t HW, int32_t groups, const void* gamma, const void* beta, float eps,

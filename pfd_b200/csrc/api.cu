@@ -33,6 +33,14 @@ int option(const char* name, int dflt) {
   auto it = opt_table().find(name);
   return it == opt_table().end() ? dflt : it->second;
 }
+
+// PFD_DETERMINISTIC=1 in the environment when the library is loaded makes deterministic mode the default, so that
+// unmodified programs can run in either mode; pfd_set_option("deterministic", v) overrides it, a reset restores it.
+static const int g_det_default = [] {
+  const char* e = getenv("PFD_DETERMINISTIC");
+  return (e && e[0] == '1') ? 1 : 0;
+}();
+bool deterministic() { return option("deterministic", g_det_default) != 0; }
 }  // namespace pfd
 
 extern "C" PFD_API int pfd_set_option(const char* name, int32_t value) {

@@ -84,4 +84,15 @@ inline int num_sms() {
   return n;
 }
 
+// Deterministic mode (pfd_set_option "deterministic"; default from PFD_DETERMINISTIC=1 at load, see api.cu): every
+// summation order depends only on a sample's own shapes, never on the batch, the SM count or a race between CTAs.
+bool deterministic();
+// SM count the GEMM and GroupNorm plan their grids and split-K with: the device's, or the smaller "plan_sms" option
+// (lets one card reproduce the plan of a smaller one).
+inline int plan_sms() {
+  const int dev = num_sms();
+  const int p = option("plan_sms", 0);
+  return (p > 0 && p < dev) ? p : dev;
+}
+
 }  // namespace pfd

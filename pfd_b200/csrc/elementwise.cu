@@ -7,6 +7,8 @@
 #include <cuda_runtime.h>
 #include <math.h>
 
+#include <mutex>
+
 #include "../../include/pfd_b200.h"
 #include "common.h"
 
@@ -150,6 +152,145 @@ gn_stats_kernel(const __half* __restrict__ x1, int c1, const __half* __restrict_
     atomicAdd(&ws[((long long)n * groups + threadIdx.x) * 2 + 0], (double)s_sum[threadIdx.x]);
     atomicAdd(&ws[((long long)n * groups + threadIdx.x) * 2 + 1], (double)s_sq[threadIdx.x]);
   }
+}
+
+// Deterministic statistics (deterministic mode).  Same per-thread accumulation as gn_stats_kernel; then
+//   1. every thread stores its 8 per-channel fp32 sums in shared memory, red[lane][channel];
+//   2. warp w folds group g (g = w, w + warps, ...): lane l adds items l, l + 32, ... of the group's (lane, channel)
+//      list in fp64, then a fixed xor butterfly -> one fp64 (sum, sumsq) partial per (image, group, chunk) in part;
+//   3. the last CTA of an image to arrive (integer counter) adds that image's partials in chunk order the same way and
+//      writes the final (sum, sumsq) to ws; it resets the counter for the next call.
+// The chunk size comes from (HW, C) alone (see pfd_groupnorm_f16), so no order depends on NB or on the SM count.
+constexpr int GN_DET_MAX_CHUNKS = 128;     // per image; ppc >= HW / 128
+constexpr int GN_DET_MAX_NB = 64;
+
+__device__ __forceinline__ double warp_sum_d(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
+__global__ void __launch_bounds__(320)
+gn_stats_det_kernel(const __half* __restrict__ x1, int c1, const __half* __restrict__ x2, int c2, long long HW,
+                    int groups, long long pix_per_cta, double2* __restrict__ part, int* __restrict__ arrivals,
+                    double* __restrict__ ws) {
+  pdl_enter();
+  extern __shared__ float red[];            // [2][lanes][C]: sums, then sums of squares
+  __shared__ int s_last;
+  const int C = c1 + c2;
+  const int cpg = C / groups;
+  const int vecs = C / 8;
+  const int n = blockIdx.y;
+  const int chunks = gridDim.x;
+  const long long p0 = (long long)blockIdx.x * pix_per_cta;
+  long long p1 = p0 + pix_per_cta;
+  if (p1 > HW) p1 = HW;
+  const int lanes = blockDim.x / vecs;
+  const int nl = lanes >= 1 ? lanes : 1;
+  float* red_s = red;
+  float* red_q = red + (long long)nl * C;
+  const long long base = (long long)n * HW;
+  if (lanes >= 1) {
+    if (threadIdx.x < lanes * vecs) {
+      const int v = threadIdx.x % vecs, lane = threadIdx.x / vecs;
+      const int c = v * 8;
+      float sm[8], sq[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) sm[i] = sq[i] = 0.f;
+      long long pix = p0 + lane;
+      for (; pix + 3 * lanes < p1; pix += 4 * lanes) {
+        uint4 u[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) u[k] = gn_load(x1, c1, x2, c2, base + pix + k * lanes, c);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          float f[8];
+          unpack8(u[k], f);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            sm[i] += f[i];
+            sq[i] += f[i] * f[i];
+          }
+        }
+      }
+      for (; pix < p1; pix += lanes) {
+        float f[8];
+        unpack8(gn_load(x1, c1, x2, c2, base + pix, c), f);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          sm[i] += f[i];
+          sq[i] += f[i] * f[i];
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        red_s[lane * C + c + i] = sm[i];
+        red_q[lane * C + c + i] = sq[i];
+      }
+    }
+  } else {
+    // very wide rows (vecs > blockDim): a thread owns vectors v, v + blockDim, ... and walks the chunk for each
+    for (int v = threadIdx.x; v < vecs; v += blockDim.x) {
+      const int c = v * 8;
+      float sm[8], sq[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) sm[i] = sq[i] = 0.f;
+      for (long long pix = p0; pix < p1; ++pix) {
+        float f[8];
+        unpack8(gn_load(x1, c1, x2, c2, base + pix, c), f);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) {
+          sm[i] += f[i];
+          sq[i] += f[i] * f[i];
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {
+        red_s[c + i] = sm[i];
+        red_q[c + i] = sq[i];
+      }
+    }
+  }
+  __syncthreads();
+  // only whole warps fold (blockDim is a multiple of vecs, not always of 32): the shuffles need all 32 lanes
+  const int warp = threadIdx.x >> 5, lid = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+  const int items = nl * cpg;                // item j = (lane j / cpg, channel g * cpg + j % cpg)
+  for (int g = warp; warp < nwarps && g < groups; g += nwarps) {
+    double s = 0.0, q = 0.0;
+    for (int j = lid; j < items; j += 32) {
+      const int idx = (j / cpg) * C + g * cpg + j % cpg;
+      s += (double)red_s[idx];
+      q += (double)red_q[idx];
+    }
+    s = warp_sum_d(s);
+    q = warp_sum_d(q);
+    if (lid == 0) {
+      part[((long long)n * groups + g) * chunks + blockIdx.x] = make_double2(s, q);
+      __threadfence();                       // the partial is visible device-wide before this CTA is counted in
+    }
+  }
+  // count this CTA in; the last arrival of image n reduces the image's partials
+  __syncthreads();
+  if (threadIdx.x == 0) s_last = atomicAdd(&arrivals[n], 1) == chunks - 1;
+  __syncthreads();
+  if (!s_last) return;
+  __threadfence();
+  for (int g = warp; warp < nwarps && g < groups; g += nwarps) {
+    const double2* pg = part + ((long long)n * groups + g) * chunks;
+    double s = 0.0, q = 0.0;
+    for (int j = lid; j < chunks; j += 32) {
+      const double2 t = __ldcg(pg + j);
+      s += t.x;
+      q += t.y;
+    }
+    s = warp_sum_d(s);
+    q = warp_sum_d(q);
+    if (lid == 0) {
+      ws[((long long)n * groups + g) * 2 + 0] = s;
+      ws[((long long)n * groups + g) * 2 + 1] = q;
+    }
+  }
+  if (threadIdx.x == 0) arrivals[n] = 0;
 }
 
 __global__ void __launch_bounds__(320)
@@ -662,6 +803,43 @@ static inline int grid_for(long long total, int threads) {
   return (int)g;
 }
 
+// Scratch of the deterministic GroupNorm statistics, one per device: GN_DET_MAX_NB arrival counters, then the fp64
+// partials [NB][groups][chunks].  Allocated (and the counters zeroed) by the first deterministic call on the device,
+// which must not be inside a stream capture - every graph-captured path of the package runs eagerly first.  The
+// counters return to zero at the end of every call, and the calls of one device are stream-ordered (like the GEMM's
+// split-K workspace), so one buffer serves them all.
+constexpr size_t GN_DET_COUNTER_BYTES = 256;
+constexpr size_t GN_DET_SCRATCH_BYTES =
+    GN_DET_COUNTER_BYTES + sizeof(double) * 2 * GN_DET_MAX_NB * GN_MAX_GROUPS * GN_DET_MAX_CHUNKS;
+static_assert(GN_DET_MAX_NB * sizeof(int) <= GN_DET_COUNTER_BYTES, "arrival counters overflow their slot");
+
+static char* gn_det_scratch(cudaStream_t st) {
+  constexpr int MAX_DEV = 64;
+  static std::mutex mu;
+  static char* buf[MAX_DEV] = {nullptr};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= MAX_DEV) return nullptr;
+  std::lock_guard<std::mutex> lk(mu);
+  if (buf[dev]) return buf[dev];
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  if (cudaStreamIsCapturing(st, &cs) != cudaSuccess || cs != cudaStreamCaptureStatusNone) {
+    (void)cudaGetLastError();
+    return nullptr;
+  }
+  char* p = nullptr;
+  if (cudaMalloc(&p, GN_DET_SCRATCH_BYTES) != cudaSuccess) {
+    (void)cudaGetLastError();
+    return nullptr;
+  }
+  if (cudaMemset(p, 0, GN_DET_COUNTER_BYTES) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) {
+    (void)cudaGetLastError();
+    cudaFree(p);
+    return nullptr;
+  }
+  buf[dev] = p;
+  return p;
+}
+
 }  // namespace pfd
 
 using namespace pfd;
@@ -681,17 +859,39 @@ extern "C" PFD_API int pfd_groupnorm_f16(const void* x1, int32_t c1, const void*
   int threads = vecs <= 320 ? (vecs <= 256 ? (256 / vecs) * vecs : vecs) : 256;
   if (threads < 64) threads = vecs * ((64 + vecs - 1) / vecs);
   const double inv_cnt = 1.0 / ((double)HW * (C / groups));
-  if (zero_ws) cudaMemsetAsync(dws, 0, sizeof(double) * 2 * NB * groups, st);
-  // ~3 CTAs per SM, but at least 16 pixels per pixel-lane so the per-CTA setup is amortised
-  long long chunks = (3LL * num_sms() + NB - 1) / NB;
-  long long ppc = (HW + chunks - 1) / chunks;
+  const bool det = deterministic();
   const long long min_ppc = 16LL * (threads / vecs > 0 ? threads / vecs : 1);
+  long long ppc;
+  if (det) {
+    // chunk size from (HW, C) only: 16 pixels per pixel-lane, but at most GN_DET_MAX_CHUNKS chunks per image
+    ppc = (HW + GN_DET_MAX_CHUNKS - 1) / GN_DET_MAX_CHUNKS;
+  } else {
+    if (zero_ws) cudaMemsetAsync(dws, 0, sizeof(double) * 2 * NB * groups, st);
+    // ~3 CTAs per SM, but at least 16 pixels per pixel-lane so the per-CTA setup is amortised
+    const long long c0 = (3LL * plan_sms() + NB - 1) / NB;
+    ppc = (HW + c0 - 1) / c0;
+  }
   if (ppc < min_ppc) ppc = min_ppc;
-  chunks = (HW + ppc - 1) / ppc;
+  const long long chunks = (HW + ppc - 1) / ppc;
   dim3 grid((unsigned)chunks, (unsigned)NB);
-  launch_k(gn_stats_kernel, dim3(grid), dim3(threads), (size_t)(0), st, static_cast<const __half*>(x1), c1, static_cast<const __half*>(x2), c2,
-                                            HW, groups, ppc, dws);
-  if (int rc = check_launch("gn_stats")) return rc;
+  if (det) {
+    const int lanes = threads / vecs > 0 ? threads / vecs : 1;
+    const size_t smem = sizeof(float) * 2 * lanes * C;
+    if (NB > GN_DET_MAX_NB || smem > 48 * 1024)
+      return set_error("pfd_groupnorm_f16: deterministic statistics support NB <= %d and C <= 6144 (NB=%d, C=%d)",
+                       GN_DET_MAX_NB, NB, C);
+    char* dscr = gn_det_scratch(st);
+    if (!dscr) return set_error("pfd_groupnorm_f16: deterministic statistics scratch unavailable (the first "
+                                "deterministic call on a device must not be inside a stream capture)");
+    launch_k(gn_stats_det_kernel, grid, dim3(threads), smem, st, static_cast<const __half*>(x1), (int)c1,
+             static_cast<const __half*>(x2), (int)c2, (long long)HW, (int)groups, (long long)ppc,
+             reinterpret_cast<double2*>(dscr + GN_DET_COUNTER_BYTES), reinterpret_cast<int*>(dscr), dws);
+    if (int rc = check_launch("gn_stats_det")) return rc;
+  } else {
+    launch_k(gn_stats_kernel, dim3(grid), dim3(threads), (size_t)(0), st, static_cast<const __half*>(x1), c1, static_cast<const __half*>(x2), c2,
+                                              HW, groups, ppc, dws);
+    if (int rc = check_launch("gn_stats")) return rc;
+  }
   launch_k(gn_apply_kernel, dim3(grid), dim3(threads), (size_t)(0), st, static_cast<const __half*>(x1), (int)c1,
            static_cast<const __half*>(x2), (int)c2, (long long)HW, (int)groups, static_cast<const __half*>(gamma),
            static_cast<const __half*>(beta), eps, (int)silu, (const double*)dws, static_cast<__half*>(out), (long long)ppc,

@@ -899,8 +899,9 @@ static int launch_gemm(GemmParams& p, int grid, cudaStream_t stream) {
   // deterministic; it trades the idle SMs of the last wave for a partial-tile hand-off through L2 per tail tile.
   p.sk_R = 0;
   p.sk_dp_tiles = 0;
-  if (p.splits == 1 && option("gemm_streamk", 0)) {
-    const int G = num_sms();
+  // deterministic mode ignores it: the K ranges of a tail tile would depend on the SM count and the tile count
+  if (p.splits == 1 && !deterministic() && option("gemm_streamk", 0)) {
+    const int G = plan_sms();
     const long long T = (long long)p.tiles_w * p.tiles_h * p.tiles_nb * p.n_tiles;
     const long long R = T % G, waves = (T + G - 1) / G;
     float* ws = splitk_workspace(stream);
@@ -1015,7 +1016,7 @@ extern "C" PFD_API int pfd_gemm_f16(const pfd_gemm_desc* d) {
   const int cands[5] = {256, 192, 160, 128, 64};
   int BNsel = 128;
   double best_cost = -1;
-  const int sms = num_sms();
+  const int sms = plan_sms();
   for (int i = 0; i < 5; ++i) {
     const int bn_c = cands[i];
     if (geglu && (d->N % bn_c)) continue;
@@ -1052,7 +1053,8 @@ extern "C" PFD_API int pfd_gemm_f16(const pfd_gemm_desc* d) {
   float* const skws = splitk_workspace(st);     // allocated by the first eager call on this device
   // ---- split-K for long-K problems that cannot fill the machine (8x8-level convs): fewer, wider N tiles
   //      (less A re-read through L2) x several K slices, fp32 partials reduced by splitk_finish_kernel.
-  if (!geglu && !d->bn_force && num_kb >= 32) {
+  //      Never in deterministic mode: whether it fires depends on M and the SM count, and it regroups the K sum.
+  if (!geglu && !d->bn_force && num_kb >= 32 && !deterministic()) {
     int bn_sk = 128;
     const int sk_cands[4] = {256, 192, 160, 128};
     for (int i = 0; i < 4; ++i)

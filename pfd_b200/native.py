@@ -154,10 +154,31 @@ def _check(rc: int, what: str) -> None:
         raise RuntimeError(f"{what} failed: {msg.decode() if msg else rc}")
 
 
+def env_flag(value: Optional[str]) -> bool:
+    """Value of an on/off environment switch (PFD_DETERMINISTIC, PFD_NO_PDL): on when it starts with '1'."""
+    return bool(value) and value[0] == "1"
+
+
+# Deterministic mode (pfd_set_option "deterministic"): the library reads PFD_DETERMINISTIC once when it is loaded and
+# uses it as the option's default; this mirror follows the option so Python can tell which mode is in effect.
+_DETERMINISTIC_DEFAULT = env_flag(os.environ.get("PFD_DETERMINISTIC"))
+_deterministic = _DETERMINISTIC_DEFAULT
+
+
+def deterministic() -> bool:
+    return _deterministic
+
+
 def set_env_option(name: Optional[str], value) -> None:
-    """Library tuning switch (pfd_set_option); name=None resets every switch to its default."""
+    """Library tuning switch (pfd_set_option); name=None resets every switch to its default.  Setting "deterministic"
+    here does not drop captured CUDA graphs; pfd_b200.set_deterministic() does."""
+    global _deterministic
     _check(load().pfd_set_option(None if name is None else name.encode(), 0 if value is None else int(value)),
            "pfd_set_option")
+    if name is None:
+        _deterministic = _DETERMINISTIC_DEFAULT
+    elif name == "deterministic":
+        _deterministic = bool(int(value or 0))
 
 
 def stream_ptr() -> int:
@@ -323,6 +344,9 @@ def bmm_nt(a: torch.Tensor, b: torch.Tensor, *, out: torch.Tensor, so, ndiv: int
 # GroupNorm statistics scratch: a ring of pre-zeroed slots per (device, stream).  `gn_reset()` zeroes the
 # whole ring with ONE memset (called at the start of every network evaluation); each groupnorm() call then
 # takes the next slot without a memset of its own.  If the ring is exhausted the call zeroes a fallback slot itself.
+# Deterministic mode uses the same slots: its per-chunk partials live in a library-owned per-device buffer, and only
+# the final (sum, sumsq) per (image, group) is written to the slot, so neither the slot size nor the per-evaluation
+# memset grows.
 _GN_SLOT_BYTES = 64 * 32 * 16 + 256    # up to 64 images x 32 groups x (sum, sumsq) fp64 (+ spare)
 _GN_SLOTS = 256
 _gn_rings = {}

@@ -2,8 +2,12 @@
 with pfd_b200/parallel.py - rank-0 SeeCoder encode -> NCCL broadcast, full-batch randn with the request seed + slice,
 all-gather of the decoded images - must reproduce the single-GPU result for the same seed.
 
-    python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29533 tools/split_check.py
+    python -m torch.distributed.run --nnodes=1 --nproc-per-node 2 --master-addr 127.0.0.1 --master-port 29533 tools/split_check.py [--deterministic]
+
+--deterministic runs every rank in deterministic mode (pfd_b200.set_deterministic) and requires the gathered batch to
+equal the single-GPU batch bit for bit.
 """
+import argparse
 import json
 import os
 import sys
@@ -16,11 +20,17 @@ sys.path.insert(0, ROOT)
 
 
 def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--deterministic", action="store_true")
+    args = ap.parse_args()
     world, rank, local = int(os.environ["WORLD_SIZE"]), int(os.environ["RANK"]), int(os.environ["LOCAL_RANK"])
     torch.cuda.set_device(local)
     dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     from pfd_b200 import DDIMSampler, get_model, model_cfg_bank, parallel as par
     from pfd_b200.weights import SCHEDULE_BUFFERS, fill_module_
+    if args.deterministic:
+        from pfd_b200 import set_deterministic
+        set_deterministic(True)
     net = get_model()(model_cfg_bank()("pfd_seecoder"))
     fill_module_(net, seed=0, skip=SCHEDULE_BUFFERS)
     net = net.half()
@@ -53,11 +63,13 @@ def main():
         rel = (diff.pow(2).mean() / single.float().pow(2).mean()).sqrt().item()
         res = {"world": world, "batch": B, "shards": [par.shard_range(B, world, r) for r in range(world)],
                "noise_slice_equals_single_gpu_randn": same_noise, "rel_rms_gathered_vs_single_gpu": rel,
-               "max_abs": diff.abs().max().item(), "shape": list(full.shape)}
+               "max_abs": diff.abs().max().item(), "shape": list(full.shape),
+               "deterministic": args.deterministic, "exact_equal": bool(torch.equal(full, single))}
         print("SPLIT_RESULT " + json.dumps(res), flush=True)
     dist.barrier()
     dist.destroy_process_group()
-    if rank == 0 and not (res["noise_slice_equals_single_gpu_randn"] and res["rel_rms_gathered_vs_single_gpu"] < 3e-3):
+    if rank == 0 and not (res["noise_slice_equals_single_gpu_randn"] and res["rel_rms_gathered_vs_single_gpu"] < 3e-3
+                          and (res["exact_equal"] or not args.deterministic)):
         sys.exit(1)
 
 
