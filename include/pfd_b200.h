@@ -71,6 +71,11 @@ PFD_API int pfd_set_option(const char* name, int32_t value);
  *   out[n, y, x, :] = act( alpha * sum_seg sum_tap sum_c A_seg[n, y*s+dy-1+o, x*s+dx-1+o, c] * Wt[:, k(seg,tap,c)]
  *                          + bias + rowadd[n, :] ) + residual[n, y, x, :]
  *
+ * Rounding: the sum is accumulated in fp32; acc*alpha + bias + rowadd and the activation are evaluated in fp32 and
+ *   rounded to fp16 once, y = fp16(act(...)); the residual is then added in fp16, out = fp16(y + residual) - the
+ *   reference's `x + f(h)` on fp16 tensors.  Every path (staged or direct epilogue, split-K finish, stream-K) rounds
+ *   at these two points, so the plan changes only the fp32 summation order of the accumulator.
+ *
  * Replaces: torch.nn.functional.conv2d / F.linear / torch.einsum / torch.bmm at
  *   openaimodel.py:203,229,240 (ResBlock convs + skip), :150 (Downsample), :105 (Upsample conv),
  *   attention.py:169-176,186-201 (to_q/k/v/out, QK^T, PV), :47,67 (GEGLU proj, ff out),

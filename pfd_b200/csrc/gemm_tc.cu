@@ -468,8 +468,7 @@ __device__ __forceinline__ void gemm_store_tile(const GemmParams& p, int tile, c
 
 // Direct epilogue from the accumulator registers, for the tiles the staged epilogue does not take:
 //   * split-K slice: raw fp32 partials -> workspace (bias etc. in splitk_finish_kernel);
-//   * element-strided outputs (V^T, !vec_ok): as gemm_stage_tile, but the residual is added in fp32 before the
-//     single rounding.
+//   * element-strided outputs (V^T, !vec_ok): as gemm_stage_tile + gemm_store_tile, with scalar stores.
 template <int BN>
 __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const float (&acc)[BN / 2], int cw, int tile,
                                               int split, int m_tiles) {
@@ -493,16 +492,17 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const float (
     row_off[i] = out_row_off(p, r);
     rowadd_row[i] = (p.rowadd && valid[i]) ? p.rowadd + (long long)r.n * p.rowadd_ld : nullptr;
   }
-  // fp16 pair (lo, hi) -> output columns c, c + 1 of row i
+  // (lo, hi) -> fp16 output columns c, c + 1 of row i; the residual is added to the fp16 values, as the store warps do
   auto store2 = [&](int i, int c, float lo, float hi) {
     const long long o0 = row_off[i] + out_col_off(p, c);
     const long long o1 = row_off[i] + out_col_off(p, c + 1);
+    __half h0 = __float2half_rn(lo), h1 = __float2half_rn(hi);
     if (p.residual) {
-      lo += __half2float(p.residual[o0]);
-      hi += __half2float(p.residual[o1]);
+      h0 = __hadd(h0, p.residual[o0]);
+      h1 = __hadd(h1, p.residual[o1]);
     }
-    p.out[o0] = __float2half_rn(lo);
-    p.out[o1] = __float2half_rn(hi);
+    p.out[o0] = h0;
+    p.out[o1] = h1;
   };
 
   if (p.splits > 1) {
@@ -769,28 +769,30 @@ splitk_finish_kernel(const __grid_constant__ GemmParams p) {
 #pragma unroll
       for (int k = 0; k < 8; ++k) acc[k] = act_apply(acc[k], p.act);
     }
+    // fp16(act(...)), then the residual added in fp16: the same rounding as the staged epilogue
     const long long row_off = (long long)(n / p.ndiv) * p.so_n1 + (long long)(n % p.ndiv) * p.so_n0 +
                               (long long)y * p.so_y + (long long)x * p.so_x;
-    const long long coff = (long long)(col / p.cdiv) * p.so_c1 + (long long)(col % p.cdiv) * p.so_c0;
     if (p.vec_ok) {
-      if (p.residual) {
-        float rv[8];
-        load8h(p.residual + row_off + coff, rv);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) acc[k] += rv[k];
-      }
+      const long long off = row_off + out_col_off(p, col);
       uint4 o;
       __half2* oh = reinterpret_cast<__half2*>(&o);
 #pragma unroll
       for (int k = 0; k < 4; ++k) oh[k] = __floats2half2_rn(acc[2 * k], acc[2 * k + 1]);
-      *reinterpret_cast<uint4*>(p.out + row_off + coff) = o;
+      if (p.residual) {
+        const uint4 r = __ldg(reinterpret_cast<const uint4*>(p.residual + off));
+        const __half2* rh = reinterpret_cast<const __half2*>(&r);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) oh[k] = __hadd2(oh[k], rh[k]);
+      }
+      *reinterpret_cast<uint4*>(p.out + off) = o;
     } else {
+      // column by column: a head width (cdiv) that is not a multiple of 8 splits the 8 columns between two heads
 #pragma unroll
       for (int k = 0; k < 8; ++k) {
-        const long long off = row_off + coff + (long long)k * p.so_c0;
-        float t = acc[k];
-        if (p.residual) t += __half2float(p.residual[off]);
-        p.out[off] = __float2half_rn(t);
+        const long long off = row_off + out_col_off(p, col + k);
+        __half h = __float2half_rn(acc[k]);
+        if (p.residual) h = __hadd(h, p.residual[off]);
+        p.out[off] = h;
       }
     }
   }
