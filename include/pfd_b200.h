@@ -243,6 +243,22 @@ PFD_API int pfd_ksampler_step_f32(const void* eps, int32_t cfg, float guidance, 
 PFD_API int pfd_ksampler_begin_step(int32_t* step, const float* ttab, int32_t nsteps, float* t_out, int32_t nb,
                                     void* stream);
 
+/*
+ * Per-sample counter-based Gaussian noise (graph-capturable):
+ *   out[b*n + e] = fp16(scale * z(seeds[b], stream_id, draw + (draw_dev ? *draw_dev : 0), e)),  b < B, e < n
+ * z is a pure function of its arguments, so sample b's noise depends on its own seed only, never on the batch:
+ *   Philox4x32-10 with key = (seed & 0xffffffff, seed >> 32) and counter = (g & 0xffffffff, g >> 32, draw, stream_id),
+ *   g = e / 4, gives the words w0..w3; Box-Muller over (w0, w1) and (w2, w3) in fp32 with the accurate device functions:
+ *     u1 = fp32(fp32(w0) + 1) * 2^-32  (in (0, 1]),   u2 = fp32(w1) * 2^-32,
+ *     z0 = sqrtf(-2 logf(u1)) * cos(2 pi u2),   z1 = sqrtf(-2 logf(u1)) * sin(2 pi u2)   (sincospif(2 u2))
+ *   and (z2, z3) likewise from (w2, w3); element e takes z_(e % 4) of group g.
+ * seeds: device array of B uint64.  draw_dev (optional): device int32 added to draw, so a captured graph can use the
+ * sampler's device-side step counter as the draw index.  Streams used by the samplers: 0 = x_T, 1 = per-step sampler
+ * noise (draw = schedule position), 2 = img2img forward noise.  Grid-stride, one Philox call per 4 elements.
+ */
+PFD_API int pfd_randn_f16(void* out, int32_t B, int64_t n, const uint64_t* seeds, uint32_t stream_id, int32_t draw,
+                          const int32_t* draw_dev, float scale, void* stream);
+
 /* Swin window plumbing on channel-last [B,H,W,C] (swin.py:269-304): pad + cyclic shift + window
  * partition in one gather (fwd) and the inverse scatter + crop (bwd). */
 PFD_API int pfd_window_gather_f16(const void* x, int32_t B, int32_t H, int32_t W, int32_t C, int32_t ws,

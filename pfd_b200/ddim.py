@@ -7,7 +7,10 @@ fused into one CUDA kernel that reproduces the reference's fp16 rounding sequenc
 The sampling loop itself lives on the device: the step counter, the timestep table and the
 coefficient table are device buffers (pfd_ddim_begin_step), so ONE captured CUDA graph holds all
 steps of a request (eta == 0) and is replayed with a single launch; the graph is cached across
-requests, keyed on shapes + a signature of the weights it baked in.
+requests, keyed on shapes + a signature of the weights it baked in.  With per-sample seeds
+(x_info["seeds"], pfd_b200/rng.py) x_T (stream 0), img2img's forward noise (stream 2) and, for eta > 0,
+every step's noise (stream 1, drawn on the device inside the graph) come from each sample's own seed,
+so the eta > 0 loop is one graph as well.
 """
 from __future__ import annotations
 
@@ -18,6 +21,7 @@ import numpy as np
 import torch
 
 from . import native as nv
+from . import rng
 from .graphs import capture as graph_capture, weights_signature
 
 
@@ -96,8 +100,8 @@ class DDIMSampler(object):
         return self.ddim_sampling(shape, x_info=x_info, c_info=c_info, noise_dropout=noise_dropout,
                                   temperature=temperature, log_every_t=log_every_t)
 
-    def _initial_latent(self, shape, x_info, dtype, timesteps):
-        """ddim.py:94-105: returns (x_T fp16, timesteps actually walked)."""
+    def _initial_latent(self, shape, x_info, dtype, timesteps, seeds=None):
+        """ddim.py:94-105: returns (x_T fp16, timesteps actually walked).  seeds: per-sample device seeds (or None)."""
         model = self.model
         device = model.device
         if x_info.get("xt", None) is not None:
@@ -108,10 +112,16 @@ class DDIMSampler(object):
             n_fwd = int(x_info["x0_forward_timesteps"])
             x0 = x_info["x0"].to(device=device, dtype=torch.float16).contiguous()
             t_fwd = int(timesteps[n_fwd])
-            noise = torch.randn_like(x0)
+            if seeds is not None:
+                noise = rng.randn_into(torch.empty_like(x0), seeds, rng.Q_SAMPLE)
+            else:
+                noise = torch.randn_like(x0)
             x_T = nv.axpby(x0, float(model.sqrt_alphas_cumprod[t_fwd]), noise,
                            float(model.sqrt_one_minus_alphas_cumprod[t_fwd]))
             return x_T, timesteps[:n_fwd]
+        if seeds is not None:
+            return rng.randn_into(torch.empty(tuple(shape), device=device, dtype=torch.float16), seeds, rng.X_T), \
+                timesteps
         # same RNG call as ddim.py:105 (dtype of the conditioning; fp16 on the GPU path)
         return torch.randn(shape, device=device, dtype=dtype).to(torch.float16), timesteps
 
@@ -125,7 +135,11 @@ class DDIMSampler(object):
         if noise_dropout > 0.0:
             raise NotImplementedError("noise_dropout is a training-time option not used by app.py")
         bs = shape[0]
-        x_T, timesteps = self._initial_latent(shape, x_info, c_info["conditioning"].dtype, self.ddim_timesteps)
+        seeds = x_info.get("seeds", None)
+        seeded = seeds is not None
+        if seeded:
+            seeds = rng.seeds_tensor(rng.parse_seeds(seeds, int(bs)), model.device)
+        x_T, timesteps = self._initial_latent(shape, x_info, c_info["conditioning"].dtype, self.ddim_timesteps, seeds)
         guidance = float(c_info["unconditional_guidance_scale"])
         cond = c_info["conditioning"]
         uncond = c_info.get("unconditional_conditioning", None)
@@ -135,8 +149,9 @@ class DDIMSampler(object):
         total = int(timesteps.shape[0])
         nb = 2 * bs if use_cfg else bs
         eta0 = eta_is_zero(self.ddim_sigmas)
+        device_noise = seeded and not eta0               # eta > 0 with seeds: the noise is drawn inside the graph
         log_idx = [i for i in range(total - 1, -1, -1) if i % log_every_t == 0 or i == total - 1]   # ddim.py:122
-        if eta0 and self.use_cuda_graph:
+        if (eta0 or device_noise) and self.use_cuda_graph:
             spg = self.steps_per_graph or total
             spg = max(1, min(spg, total))
             while total % spg:
@@ -146,18 +161,19 @@ class DDIMSampler(object):
 
         key = (tuple(x_T.shape), tuple(c_full.shape), use_cfg, guidance, c_info["type"], x_info["type"],
                None if cc is None else (tuple(cc.shape), cc.dtype), total, eta0, spg, tuple(log_idx),
-               weights_signature(model))
+               (seeded, float(temperature) if device_noise else None), weights_signature(model))
         st = self._states.get(key) if self.use_cuda_graph else None
         if st is None:
             st = _SamplerState(model, x_T, c_full, cc, nb, total, use_cfg, guidance, x_info["type"], c_info["type"],
-                               capture=self.use_cuda_graph, fused_update=eta0, steps_per_graph=spg, log_idx=log_idx)
+                               capture=self.use_cuda_graph, fused_update=eta0, steps_per_graph=spg, log_idx=log_idx,
+                               device_noise=device_noise, temperature=temperature)
             if self.use_cuda_graph:
                 if len(self._states) >= 2:
                     self._states.pop(next(iter(self._states)))
                 self._states[key] = st
         ttab = torch.as_tensor(np.ascontiguousarray(timesteps).astype(np.int64))
-        st.load_request(x_T, c_full, cc, self._coef_table()[:total], ttab)
-        if eta0:
+        st.load_request(x_T, c_full, cc, self._coef_table()[:total], ttab, seeds)
+        if eta0 or device_noise:
             st.run_all()
         else:
             for _ in range(total):
@@ -222,6 +238,8 @@ class DDIMSampler(object):
     def ddim_sampling_multicontext(self, shape, x_info, c_info_list, noise_dropout=0.0, temperature=1.0,
                                    log_every_t=100):
         """ddim.py:198-244 (eager: the mixed-context evaluation is adjacent functionality, SURVEY.md §8f)."""
+        if x_info.get("seeds", None) is not None:
+            raise NotImplementedError("x_info['seeds'] is supported by sample(), not by sample_multicontext()")
         bs = shape[0]
         x, timesteps = self._initial_latent(shape, x_info, c_info_list[0]["conditioning"].dtype, self.ddim_timesteps)
         x_info["x"] = x
@@ -270,10 +288,21 @@ class _SamplerState:
     """Static buffers + captured graphs of one sampling configuration."""
 
     def __init__(self, model, x_T, c_full, cc, nb, total, use_cfg, guidance, x_type, c_type, capture,
-                 fused_update, steps_per_graph, log_idx: List[int]):
+                 fused_update, steps_per_graph, log_idx: List[int], device_noise=False, temperature=1.0):
         dev = x_T.device
         self.model, self.use_cfg, self.guidance = model, use_cfg, guidance
         self.total, self.spg, self.fused_update = total, steps_per_graph, fused_update
+        # eta > 0 with per-sample seeds: noise drawn on the device (stream 1) before a fused update with noise
+        self.device_noise, self.temperature = device_noise, float(temperature)
+        self.seeds = torch.zeros((x_T.shape[0],), device=dev, dtype=torch.int64)
+        if device_noise:
+            self.noise = torch.zeros_like(x_T)
+            # the draw index is the schedule position k = 0, 1, ... in the order the steps run, while the DDIM step
+            # counter counts down (total-1, ..., 0): a second, ascending device counter advanced by the k-sampler's
+            # loop header (which also writes the float k, unused, to k_t) holds k
+            self.k_idx = torch.full((1,), -1, dtype=torch.int32, device=dev)
+            self.k_tab = torch.arange(total, dtype=torch.float32, device=dev)
+            self.k_t = torch.zeros((1,), dtype=torch.float32, device=dev)
         self.x = torch.empty_like(x_T)
         self.pred_x0 = torch.empty_like(x_T)
         self.eps = torch.zeros((2 * x_T.shape[0],) + tuple(x_T.shape[1:]), device=dev, dtype=torch.float16)
@@ -337,10 +366,19 @@ class _SamplerState:
         if self.fused_update:
             nv.ddim_step(e2, x, self.guidance, self.coef, self.step_idx, x, self.pred_x0, log_tab=self.log_tab,
                          log_xt=self.log_xt, log_x0=self.log_x0)
+        elif self.device_noise:
+            nv.ksampler_begin_step(self.k_idx, self.k_tab, self.k_t)
+            rng.randn_into(self.noise, self.seeds, rng.STEP, 0, self.k_idx)
+            nv.ddim_step(e2, x, self.guidance, self.coef, self.step_idx, x, self.pred_x0, noise=self.noise,
+                         temperature=self.temperature, log_tab=self.log_tab, log_xt=self.log_xt, log_x0=self.log_x0)
         else:
             self.eps.copy_(e2)                                           # eta > 0: the caller adds the noise term
 
-    def load_request(self, x_T, c_full, cc, coef, ttab):
+    def load_request(self, x_T, c_full, cc, coef, ttab, seeds=None):
+        if seeds is not None:
+            self.seeds.copy_(seeds)
+        if self.device_noise:
+            self.k_idx.fill_(-1)
         self.x.copy_(x_T)
         self.c.copy_(c_full)
         if cc is not None:

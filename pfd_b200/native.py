@@ -10,7 +10,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import POINTER, c_char_p, c_float, c_int32, c_int64, c_void_p
+from ctypes import POINTER, c_char_p, c_float, c_int32, c_int64, c_uint32, c_void_p
 from typing import Optional, Sequence, Tuple
 
 import torch
@@ -31,7 +31,7 @@ EXPORTS = [
     "pfd_flash_attn_strided_f16", "pfd_ddim_begin_step", "pfd_vae_posterior_f16",
     "pfd_canny_workspace_bytes", "pfd_canny_f32", "pfd_image_u8_roundtrip_f32",
     "pfd_hed_input_f16", "pfd_hed_pool_side_f16", "pfd_hed_fuse_f32",
-    "pfd_timestep_embedding_ft_f16", "pfd_ksampler_step_f32", "pfd_ksampler_begin_step",
+    "pfd_timestep_embedding_ft_f16", "pfd_ksampler_step_f32", "pfd_ksampler_begin_step", "pfd_randn_f16",
 ]
 PFD_KSAMPLER_NCOEF = 6
 PFD_HED_MAX_SIDES = 5
@@ -129,6 +129,7 @@ def load() -> ctypes.CDLL:
                                           c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                           c_void_p]
     lib.pfd_ksampler_begin_step.argtypes = [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_void_p]
+    lib.pfd_randn_f16.argtypes = [c_void_p, c_int32, c_int64, c_void_p, c_uint32, c_int32, c_void_p, c_float, c_void_p]
     lib.pfd_canny_workspace_bytes.argtypes = [c_int32, c_int32, c_int32]
     lib.pfd_canny_workspace_bytes.restype = c_int64
     lib.pfd_canny_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p,
@@ -541,6 +542,23 @@ def ksampler_begin_step(step: torch.Tensor, ttab: torch.Tensor, t_out: torch.Ten
         raise RuntimeError("ksampler_begin_step: step int32, ttab / t_out float32 expected")
     _check(load().pfd_ksampler_begin_step(step.data_ptr(), ttab.data_ptr(), ttab.numel(), t_out.data_ptr(),
                                           t_out.numel(), stream_ptr()), "pfd_ksampler_begin_step")
+
+
+def randn_f16(out: torch.Tensor, seeds: torch.Tensor, stream_id: int, draw: int = 0,
+              draw_dev: Optional[torch.Tensor] = None, scale: float = 1.0) -> torch.Tensor:
+    """out [B, ...] fp16 = scale * counter-based N(0, 1) noise of sample b from seeds[b] (see pfd_randn_f16).
+    seeds: CUDA int64 [B] holding the uint64 seeds' bits; draw_dev (optional): CUDA int32 [1] added to draw."""
+    _chk16(out, "randn_f16 out")
+    if not out.is_contiguous() or out.dim() < 1:
+        raise RuntimeError("randn_f16: out must be a contiguous [B, ...] tensor")
+    B = out.shape[0]
+    if seeds.dtype != torch.int64 or not seeds.is_cuda or not seeds.is_contiguous() or seeds.numel() != B:
+        raise RuntimeError(f"randn_f16: seeds must be a contiguous CUDA int64 tensor of {B} entries")
+    if draw_dev is not None and (draw_dev.dtype != torch.int32 or not draw_dev.is_cuda):
+        raise RuntimeError("randn_f16: draw_dev must be a CUDA int32 tensor")
+    _check(load().pfd_randn_f16(out.data_ptr(), B, out.numel() // B, seeds.data_ptr(), int(stream_id) & 0xffffffff,
+                                int(draw), _p(draw_dev), float(scale), stream_ptr()), "pfd_randn_f16")
+    return out
 
 
 def vae_posterior(moments: torch.Tensor, zc: int, *, noise: Optional[torch.Tensor] = None, scale: float = 1.0,

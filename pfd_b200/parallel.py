@@ -5,7 +5,9 @@ only exchanges are a broadcast of the conditioning at request start (or every ra
 reference image) and a gather of the decoded images at the end.
 
 Bit-parity with the single-GPU reference RNG stream (ddim.py:105) is kept by drawing the FULL
-[B,4,L,L] noise with the reference seed on every rank and slicing.
+[B,4,L,L] noise with the reference seed on every rank and slicing.  A request with per-sample seeds
+(x_info["seeds"], pfd_b200/rng.py) needs no such slice: each rank passes its own seeds (shard_seeds)
+and draws only its own samples' noise.
 """
 from __future__ import annotations
 
@@ -30,6 +32,18 @@ def sharded_noise(shape, seed: int, rank: int, world: int, device="cpu", dtype=t
     full = torch.randn(tuple(shape), generator=g, device=gdev, dtype=dtype)
     a, b = shard_range(shape[0], world, rank)
     return full[a:b].to(device)
+
+
+def shard_seeds(seeds, world: int, rank: int) -> List[int]:
+    """This rank's per-sample seeds: the shard_range slice of the request's full seed list (a list of ints, a
+    numpy array or an integer tensor).  Every sample's noise depends only on its own seed, so the gathered
+    images equal the single-GPU result."""
+    if torch.is_tensor(seeds):
+        vals = [int(v) for v in seeds.detach().cpu().tolist()]
+    else:
+        vals = [int(v) for v in seeds]
+    a, b = shard_range(len(vals), world, rank)
+    return vals[a:b]
 
 
 def broadcast_conditioning(c: Optional[torch.Tensor], src: int = 0, shape=None, dtype=torch.float16,

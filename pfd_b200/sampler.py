@@ -1,4 +1,5 @@
-"""k-diffusion samplers — Euler ancestral and DPM-Solver++(2M) — completing lib/model_zoo/sampler.py.
+"""k-diffusion samplers — Euler ancestral, DPM-Solver++(2M) and DPM-Solver++(2M) SDE — completing
+lib/model_zoo/sampler.py.
 
 The reference's `Sampler` (sampler.py:29-104) builds the sigma schedule from `net.alphas_cumprod` (`get_sigmas`,
 log-sigma interpolation over t = linspace(999, 0, n), then a zero appended) and holds the Euler-ancestral loop
@@ -17,8 +18,10 @@ Every step of either type is x' = a*x + b*D + c*D_prev + u*noise.  The per-step 
 float64; the update itself is one CUDA kernel (pfd_ksampler_step_f32) that keeps the state in fp32 (sigma_0 * x_T
 reaches ~60 and DPM++'s small corrections would be lost in fp16) and writes the next step's fp16 UNet input into both
 CFG halves.  The step counter and the float timestep table live on the device (pfd_ksampler_begin_step), so one
-captured CUDA graph holds the whole loop when it is deterministic (dpmpp_2m, or euler_a with eta = 0); euler_a with
-eta > 0 replays a one-step graph per step with the noise drawn on the host in between.
+captured CUDA graph holds the whole loop when it is deterministic (dpmpp_2m, or euler_a / dpmpp_2m_sde with eta = 0).
+A stochastic loop (euler_a or dpmpp_2m_sde with eta > 0) replays a one-step graph per step with the noise drawn on the
+host in between, unless the request carries per-sample seeds (x_info["seeds"], pfd_b200/rng.py): then each step's noise
+is drawn on the device from the step counter (stream 1, draw = step index) and one graph holds the whole loop too.
 """
 from __future__ import annotations
 
@@ -29,9 +32,11 @@ import numpy as np
 import torch
 
 from . import native as nv
+from . import rng
 from .graphs import capture as graph_capture, weights_signature
 
-TYPES = {"euler_a": "euler_a", "eular_a": "euler_a", "dpmpp_2m": "dpmpp_2m"}
+TYPES = {"euler_a": "euler_a", "eular_a": "euler_a", "dpmpp_2m": "dpmpp_2m", "dpmpp_2m_sde": "dpmpp_2m_sde"}
+STOCHASTIC = ("euler_a", "dpmpp_2m_sde")          # the types whose eta adds noise
 
 
 def model_log_sigmas(alphas_cumprod: torch.Tensor) -> torch.Tensor:
@@ -82,7 +87,12 @@ def coef_table(kind: str, sigmas, eta: float = 1.0) -> np.ndarray:
     x_{i+1} = a*x_i + b*D_i + c*D_{i-1} + u*noise_i, D_i = x_i - sigma_i*eps_i.
       euler_a:  x + (x - D)/sigma * (sigma_down - sigma) + sigma_up*noise (sampler.py:97-103), i.e. a = sigma_down/sigma;
       dpmpp_2m: the DPM-Solver++(2M) multistep rule in log-sigma time, first-order on the first step and on the step
-                to sigma = 0."""
+                to sigma = 0;
+      dpmpp_2m_sde: k-diffusion's sample_dpmpp_2m_sde (midpoint correction, Gaussian per-step noise): with
+                h = ln sigma - ln sigma_next, eta_h = eta*h, phi = -expm1(-h - eta_h):
+                a = (sigma_next/sigma) e^-eta_h, b = phi, c = 0, u = sigma_next sqrt(-expm1(-2 eta_h)), and from the
+                second step on (r = h_prev/h) b += phi/(2r), c = -phi/(2r); the step to sigma = 0 is x' = D.
+                eta = 0 gives dpmpp_2m's table."""
     s = np.asarray(sigmas, dtype=np.float64)
     n = len(s) - 1
     tab = np.zeros((n, nv.PFD_KSAMPLER_NCOEF), dtype=np.float64)
@@ -104,6 +114,18 @@ def coef_table(kind: str, sigmas, eta: float = 1.0) -> np.ndarray:
                     r = (math.log(s[i - 1]) - math.log(sig)) / h
                     b, c = phi * (1 + 1 / (2 * r)), -phi / (2 * r)
             u = 0.0
+        elif kind == "dpmpp_2m_sde":
+            if nxt == 0:
+                a, b, c, u = 0.0, 1.0, 0.0, 0.0
+            else:
+                h = math.log(sig) - math.log(nxt)
+                eta_h = eta * h
+                phi = -math.expm1(-h - eta_h)
+                a, b, c = nxt / sig * math.exp(-eta_h), phi, 0.0
+                u = nxt * math.sqrt(-math.expm1(-2.0 * eta_h))
+                if i > 0:
+                    r = (math.log(s[i - 1]) - math.log(sig)) / h
+                    b, c = b + 0.5 * phi / r, -0.5 * phi / r
         else:
             raise ValueError(f"unknown sampler type {kind!r}")
         tab[i] = (sig, a, b, c, u, 1.0 / math.sqrt(nxt * nxt + 1.0))
@@ -116,7 +138,8 @@ def log_steps(total: int, log_every_t: int) -> List[int]:
 
 
 class Sampler(object):
-    """Euler-ancestral ('euler_a', alias 'eular_a') / DPM-Solver++(2M) ('dpmpp_2m') sampler for the pfd nets."""
+    """Euler-ancestral ('euler_a', alias 'eular_a') / DPM-Solver++(2M) ('dpmpp_2m') / DPM-Solver++(2M) SDE
+    ('dpmpp_2m_sde') sampler for the pfd nets."""
 
     def __init__(self, net, type="euler_a", **kwargs):
         if type not in TYPES:
@@ -133,9 +156,12 @@ class Sampler(object):
     def sample(self, steps, shape, x_info, c_info, eta=1.0, sigmas: Optional[Sequence[float]] = None,
                log_every_t=100, verbose=True):
         """-> (x fp16 NCHW latent for net.vae_decode, {"pred_xt": [...], "pred_x0": [...]}).
-        eta: Euler-ancestral noise scale (1 = ancestral, 0 = plain Euler); ignored by dpmpp_2m.
+        eta: noise scale of euler_a (1 = ancestral, 0 = plain Euler) and dpmpp_2m_sde (0 = dpmpp_2m); ignored by
+             dpmpp_2m.
         sigmas: explicit descending schedule (its timesteps by sigma_to_t); default get_sigmas(steps).
-        x_info["xt"]: unit noise, scaled by sigma_0 (sampler.py:89); otherwise drawn with torch.randn."""
+        x_info["xt"]: unit noise, scaled by sigma_0 (sampler.py:89); otherwise drawn with torch.randn, or from the
+        per-sample seeds x_info["seeds"] (stream 0), which also make the per-step noise come from the device
+        (stream 1, draw = step index) inside one graph of the whole loop."""
         model = self.net
         if x_info.get("x0", None) is not None:
             raise NotImplementedError("img2img (x_info['x0']) is only available with DDIMSampler")
@@ -147,14 +173,21 @@ class Sampler(object):
             if sig.ndim != 1 or len(sig) < 2 or np.any(sig[:-1] <= 0) or np.any(np.diff(sig) >= 0):
                 raise ValueError("sigmas must be a descending schedule of at least two values, positive except the last")
             ts = sigma_to_t(sig[:-1], model_log_sigmas(model.alphas_cumprod))
-        eta = float(eta) if self.type == "euler_a" else 0.0
+        eta = float(eta) if self.type in STOCHASTIC else 0.0
         total = len(sig) - 1
         coef = coef_table(self.type, sig, eta)
-        stochastic = self.type == "euler_a" and eta != 0.0
+        stochastic = self.type in STOCHASTIC and eta != 0.0
 
         device = model.device
+        seeds = x_info.get("seeds", None)
+        seeded = seeds is not None
+        if seeded:
+            seeds = rng.seeds_tensor(rng.parse_seeds(seeds, int(shape[0])), device)
         if x_info.get("xt", None) is not None:
             xt = x_info["xt"].to(device=device)
+        elif seeded:
+            xt = torch.empty(tuple(shape), device=device, dtype=torch.float16)
+            rng.randn_into(xt, seeds, rng.X_T)
         else:
             xt = torch.randn(shape, device=device, dtype=model.get_dtype())     # sampler.py:73
         guidance = float(c_info["unconditional_guidance_scale"])
@@ -166,18 +199,18 @@ class Sampler(object):
         logs = log_steps(total, log_every_t)
 
         key = (tuple(xt.shape), tuple(c_full.shape), use_cfg, guidance, c_info["type"], x_info["type"],
-               None if cc is None else (tuple(cc.shape), cc.dtype), total, stochastic, tuple(logs),
+               None if cc is None else (tuple(cc.shape), cc.dtype), total, stochastic, seeded, tuple(logs),
                weights_signature(model))
         st = self._states.get(key) if self.use_cuda_graph else None
         if st is None:
             st = _KSamplerState(model, tuple(xt.shape), c_full, cc, use_cfg, guidance, x_info["type"], c_info["type"],
-                                total, stochastic, logs, capture=self.use_cuda_graph)
+                                total, stochastic, logs, capture=self.use_cuda_graph, seeded=seeded)
             if self.use_cuda_graph:
                 if len(self._states) >= 2:
                     self._states.pop(next(iter(self._states)))
                 self._states[key] = st
         st.load_request(xt, float(sig[0]), 1.0 / math.sqrt(sig[0] ** 2 + 1.0), c_full, cc,
-                        torch.as_tensor(coef, dtype=torch.float32), torch.as_tensor(ts, dtype=torch.float32))
+                        torch.as_tensor(coef, dtype=torch.float32), torch.as_tensor(ts, dtype=torch.float32), seeds)
         st.run(sig)
         intermediates = {"pred_xt": [st.log_xt[s].clone() for s in range(len(logs))],
                          "pred_x0": [st.log_x0[s].clone() for s in range(len(logs))]}
@@ -191,10 +224,14 @@ class _KSamplerState:
     """Static buffers + captured graphs of one sampling configuration."""
 
     def __init__(self, model, shape, c_full, cc, use_cfg, guidance, x_type, c_type, total, stochastic,
-                 logs: List[int], capture):
+                 logs: List[int], capture, seeded=False):
         dev = c_full.device
         self.model, self.use_cfg, self.guidance = model, use_cfg, guidance
         self.total, self.stochastic = total, stochastic
+        # device-drawn noise (per-sample seeds): the loop needs no host work between steps
+        self.device_noise = stochastic and seeded
+        self.host_noise = stochastic and not seeded
+        self.seeds = torch.zeros((shape[0],), device=dev, dtype=torch.int64)
         nb = 2 * shape[0] if use_cfg else shape[0]
         self.x = torch.zeros(shape, device=dev, dtype=torch.float32)
         self.d_prev = torch.zeros_like(self.x)
@@ -233,7 +270,7 @@ class _KSamplerState:
             self.step_graph = torch.cuda.CUDAGraph()
             n0 = nv.launch_count()
             with graph_capture(self.step_graph):
-                for _ in range(1 if stochastic else total):
+                for _ in range(1 if self.host_noise else total):
                     self._one_step()
             self.n_step = nv.launch_count() - n0
 
@@ -250,11 +287,15 @@ class _KSamplerState:
         nv.ksampler_begin_step(self.step_idx, self.ttab, self.t_in)
         self.x_info["x"] = self.xin
         eps = self.model.apply_model(self.x_info, self.t_in, self.c_info)
+        if self.device_noise:                      # stream 1, draw = the step index the header just advanced to
+            rng.randn_into(self.noise, self.seeds, rng.STEP, 0, self.step_idx)
         nv.ksampler_step(eps, self.use_cfg, self.guidance, self.coef, self.step_idx, self.total - 1, self.x,
                          self.d_prev, self.xin, self.out, noise=self.noise if self.stochastic else None,
                          log_tab=self.log_tab, log_xt=self.log_xt, log_x0=self.log_x0)
 
-    def load_request(self, xt, sigma0, cin0, c_full, cc, coef, ttab):
+    def load_request(self, xt, sigma0, cin0, c_full, cc, coef, ttab, seeds=None):
+        if seeds is not None:
+            self.seeds.copy_(seeds)
         self.x.copy_(xt)
         self.x.mul_(sigma0)                                              # sampler.py:89
         self.d_prev.zero_()
@@ -282,7 +323,7 @@ class _KSamplerState:
             self._one_step()
 
     def run(self, sigmas):
-        if not self.stochastic:
+        if not self.host_noise:
             if self.step_graph is not None:
                 self._step()
             else:
