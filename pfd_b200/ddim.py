@@ -4,25 +4,27 @@ maths reproduced operation for operation on the host (including the fp16-rounded
 after `net.half()`, SURVEY.md App. C #6) and the per-step CFG combine + x_{t-1} update (+ eta noise)
 fused into one CUDA kernel that reproduces the reference's fp16 rounding sequence (pfd_ddim_step_f16).
 
-The sampling loop itself lives on the device: the step counter, the timestep table and the
+The sampling loop itself lives on the device (loop.py): the step counter, the timestep table and the
 coefficient table are device buffers (pfd_ddim_begin_step), so ONE captured CUDA graph holds all
-steps of a request (eta == 0) and is replayed with a single launch; the graph is cached across
-requests, keyed on shapes + a signature of the weights it baked in.  With per-sample seeds
-(x_info["seeds"], pfd_b200/rng.py) x_T (stream 0), img2img's forward noise (stream 2) and, for eta > 0,
-every step's noise (stream 1, drawn on the device inside the graph) come from each sample's own seed,
-so the eta > 0 loop is one graph as well.
+steps of a request (eta == 0) and is replayed with a single launch (`steps_per_graph` /
+PFD_SAMPLER_STEPS_PER_GRAPH split it into shorter graphs); the graph is cached across requests, keyed
+on shapes + a signature of the weights it baked in.  With eta > 0 and no seeds, a one-step graph that
+ends in the noisy update is replayed per step, with the reference's per-step randn_like noise drawn
+on the host in between.  With per-sample seeds (x_info["seeds"], pfd_b200/rng.py) x_T (stream 0),
+img2img's forward noise (stream 2) and, for eta > 0, every step's noise (stream 1, drawn on the
+device inside the graph) come from each sample's own seed, so the eta > 0 loop is one graph as well.
 """
 from __future__ import annotations
 
 import os
-from typing import List, Optional
+from typing import List
 
 import numpy as np
 import torch
 
+from . import loop
 from . import native as nv
 from . import rng
-from .graphs import capture as graph_capture, weights_signature
 
 
 def eta_is_zero(sigmas) -> bool:
@@ -104,9 +106,7 @@ class DDIMSampler(object):
         """ddim.py:94-105: returns (x_T fp16, timesteps actually walked).  seeds: per-sample device seeds (or None)."""
         model = self.model
         device = model.device
-        if x_info.get("xt", None) is not None:
-            return x_info["xt"].to(device=device, dtype=torch.float16), timesteps
-        if x_info.get("x0", None) is not None:
+        if x_info.get("xt", None) is None and x_info.get("x0", None) is not None:
             # img2img branch (ddim.py:94-101): noise x0 forward to the n-th DDIM timestep (q_sample, pfd.py:204-207,
             # same torch.randn_like RNG call) and run only the first n timesteps of the schedule
             n_fwd = int(x_info["x0_forward_timesteps"])
@@ -119,11 +119,8 @@ class DDIMSampler(object):
             x_T = nv.axpby(x0, float(model.sqrt_alphas_cumprod[t_fwd]), noise,
                            float(model.sqrt_one_minus_alphas_cumprod[t_fwd]))
             return x_T, timesteps[:n_fwd]
-        if seeds is not None:
-            return rng.randn_into(torch.empty(tuple(shape), device=device, dtype=torch.float16), seeds, rng.X_T), \
-                timesteps
         # same RNG call as ddim.py:105 (dtype of the conditioning; fp16 on the GPU path)
-        return torch.randn(shape, device=device, dtype=dtype).to(torch.float16), timesteps
+        return loop.initial_noise(x_info, shape, seeds, device, dtype).to(torch.float16), timesteps
 
     @torch.no_grad()
     def ddim_sampling(self, shape, x_info, c_info, noise_dropout=0.0, temperature=1.0, log_every_t=100):
@@ -134,59 +131,23 @@ class DDIMSampler(object):
         model = self.model
         if noise_dropout > 0.0:
             raise NotImplementedError("noise_dropout is a training-time option not used by app.py")
-        bs = shape[0]
-        seeds = x_info.get("seeds", None)
-        seeded = seeds is not None
-        if seeded:
-            seeds = rng.seeds_tensor(rng.parse_seeds(seeds, int(bs)), model.device)
+        seeds = loop.request_seeds(x_info, shape[0], model.device)
         x_T, timesteps = self._initial_latent(shape, x_info, c_info["conditioning"].dtype, self.ddim_timesteps, seeds)
-        guidance = float(c_info["unconditional_guidance_scale"])
-        cond = c_info["conditioning"]
-        uncond = c_info.get("unconditional_conditioning", None)
-        use_cfg = not (guidance == 1.0 or uncond is None)
-        c_full = (torch.cat([uncond, cond]) if use_cfg else cond).to(torch.float16).contiguous()   # ddim.py:147
-        cc = c_info.get("control", None)
+        cfg = loop.cfg_context(c_info)
         total = int(timesteps.shape[0])
-        nb = 2 * bs if use_cfg else bs
-        eta0 = eta_is_zero(self.ddim_sigmas)
-        device_noise = seeded and not eta0               # eta > 0 with seeds: the noise is drawn inside the graph
+        stochastic = not eta_is_zero(self.ddim_sigmas)
+        seeded = seeds is not None
         log_idx = [i for i in range(total - 1, -1, -1) if i % log_every_t == 0 or i == total - 1]   # ddim.py:122
-        if (eta0 or device_noise) and self.use_cuda_graph:
-            spg = self.steps_per_graph or total
-            spg = max(1, min(spg, total))
-            while total % spg:
-                spg -= 1
-        else:
-            spg = 1
-
-        key = (tuple(x_T.shape), tuple(c_full.shape), use_cfg, guidance, c_info["type"], x_info["type"],
-               None if cc is None else (tuple(cc.shape), cc.dtype), total, eta0, spg, tuple(log_idx),
-               (seeded, float(temperature) if device_noise else None), weights_signature(model))
-        st = self._states.get(key) if self.use_cuda_graph else None
-        if st is None:
-            st = _SamplerState(model, x_T, c_full, cc, nb, total, use_cfg, guidance, x_info["type"], c_info["type"],
-                               capture=self.use_cuda_graph, fused_update=eta0, steps_per_graph=spg, log_idx=log_idx,
-                               device_noise=device_noise, temperature=temperature)
-            if self.use_cuda_graph:
-                if len(self._states) >= 2:
-                    self._states.pop(next(iter(self._states)))
-                self._states[key] = st
+        # the update bakes temperature in whenever it adds noise
+        key = loop.state_key(model, x_T, cfg, x_info, c_info, total, log_idx, stochastic, seeded,
+                             self.steps_per_graph, float(temperature) if stochastic else None)
+        st = loop.cached_state(self._states, key, self.use_cuda_graph, lambda: _DDIMState(
+            model, x_T, cfg, x_info["type"], c_info["type"], total, log_idx, stochastic, seeded, self.steps_per_graph,
+            self.use_cuda_graph, temperature))
         ttab = torch.as_tensor(np.ascontiguousarray(timesteps).astype(np.int64))
-        st.load_request(x_T, c_full, cc, self._coef_table()[:total], ttab, seeds)
-        if eta0 or device_noise:
-            st.run_all()
-        else:
-            for _ in range(total):
-                st.eps_step()                                            # begin_step + UNet -> st.eps
-                noise = torch.randn_like(st.x)                           # ddim.py:168 (noise_like)
-                nv.ddim_step(st.eps, st.x, guidance, st.coef, st.step_idx, st.x, st.pred_x0, noise=noise,
-                             temperature=temperature, log_tab=st.log_tab, log_xt=st.log_xt, log_x0=st.log_x0)
-        intermediates = {"pred_xt": [st.log_xt[s].clone() for s in range(len(log_idx))],
-                         "pred_x0": [st.log_x0[s].clone() for s in range(len(log_idx))]}
-        out = st.x.clone()
-        x_info["x"] = out
-        c_info["c"] = c_full
-        return out, intermediates
+        st.load_request(x_T, cfg.c_full, cfg.cc, self._coef_table()[:total], ttab, seeds)
+        st.run([True] * total)                                           # ddim.py:168 draws noise every step
+        return st.result(x_info, c_info, cfg.c_full)
 
     # ------------------------------------------------------------------------------------------
     def _update(self, x, eps, guidance, index, use_original_steps, temperature, noise_dropout):
@@ -284,126 +245,45 @@ class DDIMSampler(object):
         return self._update(x, eps, guidance, index, use_original_steps, temperature, noise_dropout)
 
 
-class _SamplerState:
-    """Static buffers + captured graphs of one sampling configuration."""
+class _DDIMState(loop.LoopState):
+    """fp16 latent updated in place; the step counter counts down the schedule index (total-1, ..., 0)."""
 
-    def __init__(self, model, x_T, c_full, cc, nb, total, use_cfg, guidance, x_type, c_type, capture,
-                 fused_update, steps_per_graph, log_idx: List[int], device_noise=False, temperature=1.0):
-        dev = x_T.device
-        self.model, self.use_cfg, self.guidance = model, use_cfg, guidance
-        self.total, self.spg, self.fused_update = total, steps_per_graph, fused_update
-        # eta > 0 with per-sample seeds: noise drawn on the device (stream 1) before a fused update with noise
-        self.device_noise, self.temperature = device_noise, float(temperature)
-        self.seeds = torch.zeros((x_T.shape[0],), device=dev, dtype=torch.int64)
-        if device_noise:
-            self.noise = torch.zeros_like(x_T)
+    T_DTYPE, NCOEF, WARMUP_STEP = torch.long, 4, 1
+
+    def __init__(self, model, x_T, cfg, x_type, c_type, total, log_idx: List[int], stochastic, seeded,
+                 steps_per_graph, capture, temperature):
+        self.temperature = float(temperature)
+        self.x = self.latent = torch.zeros_like(x_T)
+        self.pred_x0 = torch.zeros_like(x_T)
+        if stochastic and seeded:
             # the draw index is the schedule position k = 0, 1, ... in the order the steps run, while the DDIM step
-            # counter counts down (total-1, ..., 0): a second, ascending device counter advanced by the k-sampler's
-            # loop header (which also writes the float k, unused, to k_t) holds k
-            self.k_idx = torch.full((1,), -1, dtype=torch.int32, device=dev)
-            self.k_tab = torch.arange(total, dtype=torch.float32, device=dev)
-            self.k_t = torch.zeros((1,), dtype=torch.float32, device=dev)
-        self.x = torch.empty_like(x_T)
-        self.pred_x0 = torch.empty_like(x_T)
-        self.eps = torch.zeros((2 * x_T.shape[0],) + tuple(x_T.shape[1:]), device=dev, dtype=torch.float16)
-        self.c = torch.empty_like(c_full)
-        self.cc = None if cc is None else torch.empty_like(cc)
-        self.t_in = torch.zeros((nb,), device=dev, dtype=torch.long)
-        self.step_idx = torch.zeros(1, dtype=torch.int32, device=dev)
-        self.coef = torch.zeros((total, 4), dtype=torch.float32, device=dev)
-        self.ttab = torch.ones((total,), dtype=torch.long, device=dev)
-        nlog = max(1, len(log_idx))
-        self.log_xt = torch.zeros((nlog,) + tuple(x_T.shape), device=dev, dtype=torch.float16)
-        self.log_x0 = torch.zeros_like(self.log_xt)
-        tab = torch.full((total,), -1, dtype=torch.int32)
-        for slot, idx in enumerate(log_idx):
-            tab[idx] = slot
-        self.log_tab = tab.to(dev)
-        self.x_info = {"type": x_type}
-        self.c_info = {"type": c_type, "control": self.cc}
-        self.prep_graph = self.step_graph = None
-        self.n_prep = self.n_step = 0
-        # eager pass first: builds every packed-weight cache and validates the launch sequence
-        self.x.copy_(x_T)
-        self.c.copy_(c_full)
-        if cc is not None:
-            self.cc.copy_(cc)
-        self._prepare()
-        if capture:
-            self.step_idx.fill_(1)
-            self._one_step()                       # warm-up on scratch state (x is re-loaded per request)
-            torch.cuda.synchronize()
-            self.prep_graph = torch.cuda.CUDAGraph()
-            n0 = nv.launch_count()
-            with graph_capture(self.prep_graph):
-                self._prepare()
-            self.n_prep = nv.launch_count() - n0
-            self.step_graph = torch.cuda.CUDAGraph()
-            n0 = nv.launch_count()
-            with graph_capture(self.step_graph):
-                for _ in range(self.spg):
-                    self._one_step()
-            self.n_step = nv.launch_count() - n0
-
-    def _prepare(self):
-        prep = self.model.prepare_context(self.c, self.c_info["type"])
-        if self.cc is not None and hasattr(self.model, "ctl"):
-            prep["hint"] = self.model.ctl.hint_features(self.cc)
-        self.c_info["c"] = prep["c"]
-        self.c_info["_pfd_prepared"] = prep
+            # counter counts down: a second, ascending device counter advanced by the k-sampler's loop header (which
+            # also writes the float k, unused, to k_t) holds k
+            self.k_idx = torch.full((1,), -1, dtype=torch.int32, device=x_T.device)
+            self.k_tab = torch.arange(total, dtype=torch.float32, device=x_T.device)
+            self.k_t = torch.zeros((1,), dtype=torch.float32, device=x_T.device)
+        super().__init__(model, tuple(x_T.shape), cfg, x_type, c_type, total, log_idx, stochastic, seeded,
+                         steps_per_graph, capture)
 
     def _one_step(self):
         # device-side loop header (index -= 1, t = timesteps[index]; ddim.py:111-113) -> CFG batch (ddim.py:145-150)
-        # -> UNet (+ControlNet) -> [fused CFG combine + DDIM update, in place on x]
+        # -> UNet (+ControlNet) -> fused CFG combine + DDIM update (+ noise), in place on x
         nv.ddim_begin_step(self.step_idx, self.ttab, self.t_in)
         x = self.x
         self.x_info["x"] = torch.cat([x, x]) if self.use_cfg else x
         eps = self.model.apply_model(self.x_info, self.t_in, self.c_info)
-        if self.use_cfg:
-            e2 = eps
-        else:                                                            # e_t = eps * scale (ddim.py:143-144)
-            e2 = torch.cat([torch.zeros_like(eps), eps])
-        if self.fused_update:
-            nv.ddim_step(e2, x, self.guidance, self.coef, self.step_idx, x, self.pred_x0, log_tab=self.log_tab,
-                         log_xt=self.log_xt, log_x0=self.log_x0)
-        elif self.device_noise:
+        if not self.use_cfg:                                             # e_t = eps * scale (ddim.py:143-144)
+            eps = torch.cat([torch.zeros_like(eps), eps])
+        if self.device_noise:
             nv.ksampler_begin_step(self.k_idx, self.k_tab, self.k_t)
             rng.randn_into(self.noise, self.seeds, rng.STEP, 0, self.k_idx)
-            nv.ddim_step(e2, x, self.guidance, self.coef, self.step_idx, x, self.pred_x0, noise=self.noise,
-                         temperature=self.temperature, log_tab=self.log_tab, log_xt=self.log_xt, log_x0=self.log_x0)
-        else:
-            self.eps.copy_(e2)                                           # eta > 0: the caller adds the noise term
+        nv.ddim_step(eps, x, self.guidance, self.coef, self.step_idx, x, self.pred_x0,
+                     noise=self.noise if self.stochastic else None, temperature=self.temperature,
+                     log_tab=self.log_tab, log_xt=self.log_xt, log_x0=self.log_x0)
 
     def load_request(self, x_T, c_full, cc, coef, ttab, seeds=None):
-        if seeds is not None:
-            self.seeds.copy_(seeds)
+        self.x.copy_(x_T)
+        self.step_idx.fill_(self.total)
         if self.device_noise:
             self.k_idx.fill_(-1)
-        self.x.copy_(x_T)
-        self.c.copy_(c_full)
-        if cc is not None:
-            self.cc.copy_(cc)
-        self.coef.copy_(coef, non_blocking=True)
-        self.ttab.copy_(ttab, non_blocking=True)
-        self.step_idx.fill_(self.total)
-        if self.prep_graph is not None:
-            self.prep_graph.replay()
-            nv.note_replay(self.n_prep)
-        else:
-            self._prepare()
-
-    def run_all(self):
-        if self.step_graph is not None:
-            for _ in range(self.total // self.spg):
-                self.step_graph.replay()
-                nv.note_replay(self.n_step)
-        else:
-            for _ in range(self.total):
-                self._one_step()
-
-    def eps_step(self):
-        if self.step_graph is not None:
-            self.step_graph.replay()
-            nv.note_replay(self.n_step)
-        else:
-            self._one_step()
+        super().load_request(c_full, cc, coef, ttab, seeds)

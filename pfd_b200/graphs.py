@@ -1,12 +1,11 @@
 """CUDA-graph caching for fixed-shape pieces of the pipeline (SeeCoder encode, VAE decode, the
-per-step UNet evaluation).  The pipeline launches ~600 kernels per UNet evaluation and ~1100 per
+sampling loops of loop.py).  The pipeline launches ~600 kernels per UNet evaluation and ~1100 per
 SeeCoder encode; replaying captured graphs removes the Python / ctypes / tensor-map-encode cost from
 the request path.  Graphs are keyed on input shapes and on a signature of the weights they baked in
 (storage pointer + version of every parameter), so load_state_dict / .half() / .to() invalidate them.
 """
 from __future__ import annotations
 
-import contextlib
 import gc
 from typing import Callable, Dict, Hashable, List, Sequence, Tuple
 
@@ -16,20 +15,31 @@ import torch.nn as nn
 from . import native as nv
 
 
-@contextlib.contextmanager
-def capture(graph: "torch.cuda.CUDAGraph"):
-    """torch.cuda.graph(graph) with the Python garbage collector held off: a cyclic-garbage sweep in the middle of a
-    capture may run the destructor of an older CUDAGraph (cudaGraphExecDestroy), which is illegal while a stream
-    is capturing in the global capture mode and invalidates the capture."""
-    gc.collect()
-    was = gc.isenabled()
-    gc.disable()
-    try:
-        with torch.cuda.graph(graph):
-            yield
-    finally:
-        if was:
-            gc.enable()
+class CapturedGraph:
+    """fn() captured into a CUDA graph, with the library kernels it launched counted so that every replay adds them
+    to nv.launch_count().  replay() returns fn's output of the capture, which each replay rewrites in place.
+    The Python garbage collector is held off during the capture: a cyclic-garbage sweep in the middle of a capture may
+    run the destructor of an older CUDAGraph (cudaGraphExecDestroy), which is illegal while a stream is capturing in
+    the global capture mode and invalidates the capture."""
+
+    def __init__(self, fn: Callable):
+        self.graph = torch.cuda.CUDAGraph()
+        gc.collect()
+        was = gc.isenabled()
+        gc.disable()
+        n0 = nv.launch_count()
+        try:
+            with torch.cuda.graph(self.graph):
+                self.out = fn()
+        finally:
+            if was:
+                gc.enable()
+        self.n_kernels = nv.launch_count() - n0
+
+    def replay(self):
+        self.graph.replay()
+        nv.note_replay(self.n_kernels)
+        return self.out
 
 
 _generation = 0
@@ -85,18 +95,12 @@ class GraphedFunction:
         # eager warm-up builds every lazily packed weight / mask so capture sees only kernel launches
         self.first_out = fn(*self.static_in)
         torch.cuda.synchronize()
-        self.graph = torch.cuda.CUDAGraph()
-        n0 = nv.launch_count()
-        with capture(self.graph):
-            self.static_out = fn(*self.static_in)
-        self.n_kernels = nv.launch_count() - n0
+        self.graph = CapturedGraph(lambda: fn(*self.static_in))
 
     def __call__(self, *inputs: torch.Tensor):
         for s, t in zip(self.static_in, inputs):
             s.copy_(t, non_blocking=True)
-        self.graph.replay()
-        nv.note_replay(self.n_kernels)
-        return self.static_out
+        return self.graph.replay()
 
 
 class GraphCache:

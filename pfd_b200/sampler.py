@@ -22,6 +22,7 @@ captured CUDA graph holds the whole loop when it is deterministic (dpmpp_2m, or 
 A stochastic loop (euler_a or dpmpp_2m_sde with eta > 0) replays a one-step graph per step with the noise drawn on the
 host in between, unless the request carries per-sample seeds (x_info["seeds"], pfd_b200/rng.py): then each step's noise
 is drawn on the device from the step counter (stream 1, draw = step index) and one graph holds the whole loop too.
+The loop engine, shared with DDIMSampler, is loop.py.
 """
 from __future__ import annotations
 
@@ -31,9 +32,9 @@ from typing import List, Optional, Sequence
 import numpy as np
 import torch
 
+from . import loop
 from . import native as nv
 from . import rng
-from .graphs import capture as graph_capture, weights_signature
 
 TYPES = {"euler_a": "euler_a", "eular_a": "euler_a", "dpmpp_2m": "dpmpp_2m", "dpmpp_2m_sde": "dpmpp_2m_sde"}
 STOCHASTIC = ("euler_a", "dpmpp_2m_sde")          # the types whose eta adds noise
@@ -178,108 +179,36 @@ class Sampler(object):
         coef = coef_table(self.type, sig, eta)
         stochastic = self.type in STOCHASTIC and eta != 0.0
 
-        device = model.device
-        seeds = x_info.get("seeds", None)
+        seeds = loop.request_seeds(x_info, shape[0], model.device)
+        xt = loop.initial_noise(x_info, shape, seeds, model.device, model.get_dtype())     # sampler.py:73
+        cfg = loop.cfg_context(c_info)
         seeded = seeds is not None
-        if seeded:
-            seeds = rng.seeds_tensor(rng.parse_seeds(seeds, int(shape[0])), device)
-        if x_info.get("xt", None) is not None:
-            xt = x_info["xt"].to(device=device)
-        elif seeded:
-            xt = torch.empty(tuple(shape), device=device, dtype=torch.float16)
-            rng.randn_into(xt, seeds, rng.X_T)
-        else:
-            xt = torch.randn(shape, device=device, dtype=model.get_dtype())     # sampler.py:73
-        guidance = float(c_info["unconditional_guidance_scale"])
-        cond = c_info["conditioning"]
-        uncond = c_info.get("unconditional_conditioning", None)
-        use_cfg = not (guidance == 1.0 or uncond is None)
-        c_full = (torch.cat([uncond, cond]) if use_cfg else cond).to(torch.float16).contiguous()
-        cc = c_info.get("control", None)
         logs = log_steps(total, log_every_t)
-
-        key = (tuple(xt.shape), tuple(c_full.shape), use_cfg, guidance, c_info["type"], x_info["type"],
-               None if cc is None else (tuple(cc.shape), cc.dtype), total, stochastic, seeded, tuple(logs),
-               weights_signature(model))
-        st = self._states.get(key) if self.use_cuda_graph else None
-        if st is None:
-            st = _KSamplerState(model, tuple(xt.shape), c_full, cc, use_cfg, guidance, x_info["type"], c_info["type"],
-                                total, stochastic, logs, capture=self.use_cuda_graph, seeded=seeded)
-            if self.use_cuda_graph:
-                if len(self._states) >= 2:
-                    self._states.pop(next(iter(self._states)))
-                self._states[key] = st
-        st.load_request(xt, float(sig[0]), 1.0 / math.sqrt(sig[0] ** 2 + 1.0), c_full, cc,
+        key = loop.state_key(model, xt, cfg, x_info, c_info, total, logs, stochastic, seeded)
+        st = loop.cached_state(self._states, key, self.use_cuda_graph, lambda: _KSamplerState(
+            model, tuple(xt.shape), cfg, x_info["type"], c_info["type"], total, logs, stochastic, seeded,
+            self.use_cuda_graph))
+        st.load_request(xt, float(sig[0]), 1.0 / math.sqrt(sig[0] ** 2 + 1.0), cfg.c_full, cfg.cc,
                         torch.as_tensor(coef, dtype=torch.float32), torch.as_tensor(ts, dtype=torch.float32), seeds)
-        st.run(sig)
-        intermediates = {"pred_xt": [st.log_xt[s].clone() for s in range(len(logs))],
-                         "pred_x0": [st.log_x0[s].clone() for s in range(len(logs))]}
-        out = st.out.clone()
-        x_info["x"] = out
-        c_info["c"] = c_full
-        return out, intermediates
+        # sampler.py:102-103: one randn_like(x) per step with sigma_next > 0 (x is in the net's dtype)
+        st.run(sig[1:] > 0)
+        return st.result(x_info, c_info, cfg.c_full)
 
 
-class _KSamplerState:
-    """Static buffers + captured graphs of one sampling configuration."""
+class _KSamplerState(loop.LoopState):
+    """fp32 state x, the previous step's denoised D_prev, and the fp16 UNet input / output the update writes; the step
+    counter counts up (0, ..., total-1)."""
 
-    def __init__(self, model, shape, c_full, cc, use_cfg, guidance, x_type, c_type, total, stochastic,
-                 logs: List[int], capture, seeded=False):
-        dev = c_full.device
-        self.model, self.use_cfg, self.guidance = model, use_cfg, guidance
-        self.total, self.stochastic = total, stochastic
-        # device-drawn noise (per-sample seeds): the loop needs no host work between steps
-        self.device_noise = stochastic and seeded
-        self.host_noise = stochastic and not seeded
-        self.seeds = torch.zeros((shape[0],), device=dev, dtype=torch.int64)
-        nb = 2 * shape[0] if use_cfg else shape[0]
+    T_DTYPE, NCOEF, WARMUP_STEP = torch.float32, nv.PFD_KSAMPLER_NCOEF, -1
+
+    def __init__(self, model, shape, cfg, x_type, c_type, total, logs: List[int], stochastic, seeded, capture):
+        dev = cfg.c_full.device
+        nb = 2 * shape[0] if cfg.use_cfg else shape[0]
         self.x = torch.zeros(shape, device=dev, dtype=torch.float32)
         self.d_prev = torch.zeros_like(self.x)
-        self.out = torch.zeros(shape, device=dev, dtype=torch.float16)
-        self.noise = torch.zeros(shape, device=dev, dtype=torch.float16)
+        self.out = self.latent = torch.zeros(shape, device=dev, dtype=torch.float16)
         self.xin = torch.zeros((nb,) + tuple(shape[1:]), device=dev, dtype=torch.float16)
-        self.c = torch.empty_like(c_full)
-        self.cc = None if cc is None else torch.empty_like(cc)
-        self.t_in = torch.zeros((nb,), device=dev, dtype=torch.float32)
-        self.step_idx = torch.full((1,), -1, dtype=torch.int32, device=dev)
-        self.coef = torch.zeros((total, nv.PFD_KSAMPLER_NCOEF), dtype=torch.float32, device=dev)
-        self.ttab = torch.zeros((total,), dtype=torch.float32, device=dev)
-        self.log_xt = torch.zeros((max(1, len(logs)),) + tuple(shape), device=dev, dtype=torch.float16)
-        self.log_x0 = torch.zeros_like(self.log_xt)
-        tab = torch.full((total,), -1, dtype=torch.int32)
-        for slot, k in enumerate(logs):
-            tab[k] = slot
-        self.log_tab = tab.to(dev)
-        self.x_info = {"type": x_type}
-        self.c_info = {"type": c_type, "control": self.cc}
-        self.prep_graph = self.step_graph = None
-        self.n_prep = self.n_step = 0
-        # eager pass first: builds every packed-weight cache and validates the launch sequence
-        self.c.copy_(c_full)
-        if cc is not None:
-            self.cc.copy_(cc)
-        self._prepare()
-        if capture:
-            self._one_step()                       # warm-up on scratch state (everything is re-loaded per request)
-            torch.cuda.synchronize()
-            self.prep_graph = torch.cuda.CUDAGraph()
-            n0 = nv.launch_count()
-            with graph_capture(self.prep_graph):
-                self._prepare()
-            self.n_prep = nv.launch_count() - n0
-            self.step_graph = torch.cuda.CUDAGraph()
-            n0 = nv.launch_count()
-            with graph_capture(self.step_graph):
-                for _ in range(1 if self.host_noise else total):
-                    self._one_step()
-            self.n_step = nv.launch_count() - n0
-
-    def _prepare(self):
-        prep = self.model.prepare_context(self.c, self.c_info["type"])
-        if self.cc is not None and hasattr(self.model, "ctl"):
-            prep["hint"] = self.model.ctl.hint_features(self.cc)
-        self.c_info["c"] = prep["c"]
-        self.c_info["_pfd_prepared"] = prep
+        super().__init__(model, shape, cfg, x_type, c_type, total, logs, stochastic, seeded, None, capture)
 
     def _one_step(self):
         # device-side loop header (step += 1, t = t(sigma_step)) -> UNet (+ControlNet) on the fp16 input x*c_in that
@@ -294,8 +223,6 @@ class _KSamplerState:
                          log_tab=self.log_tab, log_xt=self.log_xt, log_x0=self.log_x0)
 
     def load_request(self, xt, sigma0, cin0, c_full, cc, coef, ttab, seeds=None):
-        if seeds is not None:
-            self.seeds.copy_(seeds)
         self.x.copy_(xt)
         self.x.mul_(sigma0)                                              # sampler.py:89
         self.d_prev.zero_()
@@ -303,36 +230,5 @@ class _KSamplerState:
         self.xin[:b].copy_(self.x * cin0)
         if self.use_cfg:
             self.xin[b:].copy_(self.xin[:b])
-        self.c.copy_(c_full)
-        if cc is not None:
-            self.cc.copy_(cc)
-        self.coef.copy_(coef, non_blocking=True)
-        self.ttab.copy_(ttab, non_blocking=True)
         self.step_idx.fill_(-1)
-        if self.prep_graph is not None:
-            self.prep_graph.replay()
-            nv.note_replay(self.n_prep)
-        else:
-            self._prepare()
-
-    def _step(self):
-        if self.step_graph is not None:
-            self.step_graph.replay()
-            nv.note_replay(self.n_step)
-        else:
-            self._one_step()
-
-    def run(self, sigmas):
-        if not self.host_noise:
-            if self.step_graph is not None:
-                self._step()
-            else:
-                for _ in range(self.total):
-                    self._one_step()
-            return
-        for i in range(self.total):
-            if sigmas[i + 1] > 0:
-                # sampler.py:102-103: one randn_like(x) per step with sigma_next > 0 (x is in the net's dtype);
-                # normal_ on the static buffer draws the same values from the same generator
-                self.noise.normal_()
-            self._step()
+        super().load_request(c_full, cc, coef, ttab, seeds)

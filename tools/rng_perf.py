@@ -1,7 +1,7 @@
 """Time seeded (per-sample, on-device noise) against unseeded stochastic sampling at the size of bench.py's config 2
 (64x64 latents, batch 4, CFG scale 2, synthetic weights), and the noise kernel alone:
   - DDIM-50 eta 0 (one graph for the whole loop), the per-step cost a seeded stochastic loop is compared with;
-  - DDIM-50 eta 1: unseeded (eager loop, host randn per step) vs seeded (one graph for the whole loop);
+  - DDIM-50 eta 1: unseeded (one-step graph + host noise per step) vs seeded (one graph for the whole loop);
   - euler_a-50 eta 1: unseeded (one-step graph + host noise per step) vs seeded (one graph);
   - dpmpp_2m_sde at 20 and 25 steps, eta 1, unseeded vs seeded;
   - pfd_randn_f16 at [4, 4, 64, 64] (CUDA events around a graph of 200 back-to-back launches).

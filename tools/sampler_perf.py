@@ -1,6 +1,7 @@
 """Time the samplers at the size of bench.py's config 2 (512x512 output = 64x64 latents, batch 4, CFG scale 2, i.e. a
-CFG batch of 8 per UNet evaluation) with synthetic weights: DDIM-50, euler_a-50 (eta 1: one graph replay plus one
-host noise draw per step), euler_a-50 with eta 0 and dpmpp_2m-20 / 25 (one graph for the whole loop).  Reported per
+CFG batch of 8 per UNet evaluation) with synthetic weights: DDIM-50 (eta 0: one graph for the whole loop), euler_a-50
+(eta 1: one graph replay plus one host noise draw per step, as DDIM with eta > 0 and no seeds runs), euler_a-50 with
+eta 0 and dpmpp_2m-20 / 25 (one graph for the whole loop).  Reported per
 sampler: ms per sample() call (the denoising loop only: no SeeCoder, no VAE), ms per step, latents per second, and
 the k-sampler update kernel's own time (CUDA events around a graph of 200 back-to-back launches).  The card's name and
 power limit are read in the same run.
