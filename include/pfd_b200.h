@@ -341,6 +341,30 @@ PFD_API int pfd_hed_pool_side_f16(const void* x, int32_t B, int32_t h, int32_t w
 PFD_API int pfd_hed_fuse_f32(const float* const* sides, const int32_t* side_h, const int32_t* side_w, int32_t nsides,
                              int32_t B, int32_t H, int32_t W, float inv_scale, float* out, void* stream);
 
+/*
+ * ControlNet.preprocess(type='scribble') (controlnet.py:432-491) for a whole batch; out is float32 [B,3,H,W] with 1.0
+ * on scribble pixels in all three channels (ToTensor + repeat).  Asynchronous on `stream` and graph-capturable.
+ *
+ * pfd_scribble_hed_f32: make_scribble (controlnet.py:436-454) of the HED levels round(255 * hed[n*img_stride + y*W+x])
+ *   (channel 0 of pfd_hed_fuse_f32's output with img_stride = 3*H*W): float32 cv2.GaussianBlur sigma 3 (ksize 25,
+ *   BORDER_REFLECT_101), kept where it equals cv2.dilate along one of the four 3-tap lines, `> 127` -> 255 into
+ *   nms (device uint8 [B,H,W], caller-allocated), then pfd_scribble_blur_u8 of nms into out.
+ * pfd_scribble_blur_u8: cv2.GaussianBlur(z, (0,0), 3) of a uint8 [B,H,W] map on OpenCV's fixed-point path (ksize 19,
+ *   bit-exact); writes the blurred map to `blurred` and / or `> 4` -> 1.0 to `out` (either may be NULL, not both).
+ * pfd_scribble_xdog_f32: the xdog branch (controlnet.py:476-482) on an NCHW [B,3,H,W] image in [0,1] (fp16 or fp32,
+ *   quantised like ToPILImage): per channel float32 Gaussian blurs g1 (sigma 0.5, ksize 5) and g2 (sigma 5, ksize 41),
+ *   dog = uint8(clip(255 - min_c(g2 - g1), 0, 255)) truncated, edge where uint8(2 * uint8(255 - dog)) > threshold
+ *   (the product wraps mod 256, as in the numpy expression).
+ * The float blurs use OpenCV's float32 taps but not its operation order: decisions within float32 rounding of a tie may
+ * differ from cv2 (README, scribble annotators).
+ */
+PFD_API int pfd_scribble_hed_f32(const float* hed, int64_t img_stride, int32_t B, int32_t H, int32_t W, uint8_t* nms,
+                                 float* out, void* stream);
+PFD_API int pfd_scribble_blur_u8(const uint8_t* z, int32_t B, int32_t H, int32_t W, uint8_t* blurred, float* out,
+                                 void* stream);
+PFD_API int pfd_scribble_xdog_f32(const void* x, int32_t src_is_f32, int32_t B, int32_t H, int32_t W, int32_t threshold,
+                                  float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -5,8 +5,8 @@ Same constructor arguments / state-dict keys as the reference (spatial-transform
 ``UNetModel2D_Next.apply(control=...)``.  The hint stem (controlnet.py:165-181) depends only on the
 control image, so its output is cached per hint tensor instead of being recomputed every DDIM step.
 ``preprocess`` provides the annotator-free types on the GPU ('input', 'canny' — bit-exact cv2.Canny,
-SURVEY.md §8 f1) and the HED soft-edge network ('hed', 'softedge_v11p', hed.py); the other annotator networks
-(controlnet.py:361-503) are not implemented.
+SURVEY.md §8 f1), the HED soft-edge network ('hed', 'softedge_v11p', hed.py) and the scribble maps of methods 'hed'
+and 'xdog' (scribble.py); the other annotator networks (controlnet.py:361-503) are not implemented.
 """
 from __future__ import annotations
 
@@ -167,9 +167,11 @@ class ControlNet(nn.Module):
         """controlnet.py:332-376 on the GPU: 'none', 'input' / 'shuffle_v11e' (the uint8 round trip of ToPILImage ->
         ToTensor), 'canny' / 'canny_v11p' (cv2.Canny(rgb_u8, low, high), reproduced bit-exactly by pfd_canny_f32) and
         'hed' / 'softedge_v11p' (the HED network of controlnet_annotator/hed in fp16 with fp32 accumulation, whole
-        batch at once; weights from pfd_b200.hed.load_hed / set_network, see hed.py).  x: [B,3,H,W] tensor in [0,1]
-        or an image path.  Returns float32 [B,3,H,W] on x's device; `size=` is ignored, as in the reference.  The
-        other annotator networks (midas, mlsd, openpose, pidinet, ...) raise NotImplementedError."""
+        batch at once; weights from pfd_b200.hed.load_hed / set_network, see hed.py) and 'scribble' with
+        method='hed' (HED, then make_scribble) or method='xdog' (threshold=32), see scribble.py.  x: [B,3,H,W] tensor
+        in [0,1] or an image path.  Returns float32 [B,3,H,W] on x's device; `size=` is ignored, as in the reference.
+        The other annotator networks (midas, mlsd, openpose, and pidinet, the default scribble method) raise
+        NotImplementedError; an unknown scribble method raises ValueError."""
         if type == "none" or type is None:
             return None
         if isinstance(x, str):
@@ -195,8 +197,12 @@ class ControlNet(nn.Module):
         if type in ("hed", "softedge_v11p"):
             from .hed import preprocess_hed
             return preprocess_hed(x)
+        if type == "scribble":
+            from .scribble import preprocess_scribble
+            return preprocess_scribble(x, kwargs.pop("method", "pidinet"), kwargs.pop("threshold", 32))
         raise NotImplementedError(f"controlnet annotator '{type}' is not implemented in pfd_b200 (the GPU serves "
-                                  "'input', 'canny' and 'hed'); feed a ready control map (do_preprocess=False)")
+                                  "'input', 'canny', 'hed' and 'scribble'); feed a ready control map "
+                                  "(do_preprocess=False)")
 
     def get_device(self):
         return self.time_embed[0].weight.device

@@ -32,6 +32,7 @@ EXPORTS = [
     "pfd_canny_workspace_bytes", "pfd_canny_f32", "pfd_image_u8_roundtrip_f32",
     "pfd_hed_input_f16", "pfd_hed_pool_side_f16", "pfd_hed_fuse_f32",
     "pfd_timestep_embedding_ft_f16", "pfd_ksampler_step_f32", "pfd_ksampler_begin_step", "pfd_randn_f16",
+    "pfd_scribble_hed_f32", "pfd_scribble_blur_u8", "pfd_scribble_xdog_f32",
 ]
 PFD_KSAMPLER_NCOEF = 6
 PFD_HED_MAX_SIDES = 5
@@ -141,6 +142,9 @@ def load() -> ctypes.CDLL:
                                           c_void_p, c_void_p]
     lib.pfd_hed_fuse_f32.argtypes = [POINTER(c_void_p), POINTER(c_int32), POINTER(c_int32), c_int32, c_int32, c_int32,
                                      c_int32, c_float, c_void_p, c_void_p]
+    lib.pfd_scribble_hed_f32.argtypes = [c_void_p, c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]
+    lib.pfd_scribble_blur_u8.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]
+    lib.pfd_scribble_xdog_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]
     for name in EXPORTS:
         if hasattr(lib, name) and name not in ("pfd_version", "pfd_last_error", "pfd_launch_count",
                                                "pfd_canny_workspace_bytes"):
@@ -652,6 +656,48 @@ def hed_fuse(sides: Sequence[torch.Tensor], H: int, W: int, inv_scale: float = 1
     ws = (c_int32 * n)(*[s.shape[2] for s in sides])
     _check(load().pfd_hed_fuse_f32(ptrs, hs, ws, n, B, H, W, float(inv_scale), out.data_ptr(), stream_ptr()),
            "pfd_hed_fuse_f32")
+    return out
+
+
+def scribble_hed(hed: torch.Tensor, return_nms: bool = False):
+    """make_scribble of the HED map: float32 [B,3,H,W] (pfd_hed_fuse_f32's output; channel 0 is read as the levels
+    round(255 * v)) -> float32 [B,3,H,W] scribble map (pfd_scribble_hed_f32).  return_nms=True also returns the uint8
+    [B,H,W] map after the non-maximum suppression and the `> 127` threshold."""
+    _chk32(hed, "scribble_hed")
+    if hed.dim() != 4 or hed.shape[1] < 1:
+        raise RuntimeError(f"scribble_hed: expected [B,C,H,W], got {tuple(hed.shape)}")
+    B, C, H, W = hed.shape
+    nms = torch.empty((B, H, W), device=hed.device, dtype=torch.uint8)
+    out = torch.empty((B, 3, H, W), device=hed.device, dtype=torch.float32)
+    _check(load().pfd_scribble_hed_f32(hed.data_ptr(), C * H * W, B, H, W, nms.data_ptr(), out.data_ptr(),
+                                       stream_ptr()), "pfd_scribble_hed_f32")
+    return (out, nms) if return_nms else out
+
+
+def scribble_blur_u8(z: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """cv2.GaussianBlur(z, (0,0), 3) of a CUDA uint8 [B,H,W] map, bit-exact -> (blurred uint8 [B,H,W], float32
+    [B,3,H,W] with 1.0 where blurred > 4) (pfd_scribble_blur_u8)."""
+    if z.dim() != 3 or z.dtype != torch.uint8 or not z.is_cuda:
+        raise RuntimeError(f"scribble_blur_u8: expected a CUDA uint8 [B,H,W] map, got {tuple(z.shape)} {z.dtype}")
+    z = z.contiguous()
+    B, H, W = z.shape
+    blurred = torch.empty_like(z)
+    out = torch.empty((B, 3, H, W), device=z.device, dtype=torch.float32)
+    _check(load().pfd_scribble_blur_u8(z.data_ptr(), B, H, W, blurred.data_ptr(), out.data_ptr(), stream_ptr()),
+           "pfd_scribble_blur_u8")
+    return blurred, out
+
+
+def scribble_xdog(x: torch.Tensor, threshold: int = 32) -> torch.Tensor:
+    """The xdog scribble of an NCHW [B,3,H,W] image in [0,1] (fp16/fp32) -> float32 [B,3,H,W]
+    (pfd_scribble_xdog_f32).  threshold: integer; the uint8 edge strength is compared with `>`."""
+    if x.dim() != 4 or x.shape[1] != 3 or not x.is_cuda or x.dtype not in (torch.float16, torch.float32):
+        raise RuntimeError(f"scribble_xdog: expected a CUDA fp16/fp32 [B,3,H,W] image, got {tuple(x.shape)} {x.dtype}")
+    x = x.contiguous()
+    B, _, H, W = x.shape
+    out = torch.empty((B, 3, H, W), device=x.device, dtype=torch.float32)
+    _check(load().pfd_scribble_xdog_f32(x.data_ptr(), int(x.dtype == torch.float32), B, H, W, int(threshold),
+                                        out.data_ptr(), stream_ptr()), "pfd_scribble_xdog_f32")
     return out
 
 
