@@ -90,6 +90,9 @@ struct GemmCfg {
   static constexpr int CONSUMER_REGS = BN >= 256 ? 224 : 208;
   static constexpr int PRODUCER_REGS = BN >= 256 ? 56 : 88;
   static constexpr int STORE_BATCH = BN >= 256 ? 4 : 8;
+  // The consumers load a tile's bias before its K loop, so the latency lies under the MMAs.  Not at BN = 256: 128
+  // accumulators plus 32 bias registers spill within CONSUMER_REGS, so there the loads follow the MMAs.
+  static constexpr bool BIAS_EARLY = BN < 256;
   static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS == GEMM_THREADS * 168, "register budgets");
   static_assert(STAGE_B_BYTES % 1024 == 0, "B stage must keep 1024-B swizzle alignment");
   static_assert(BN % 16 == 0 && BN >= 16 && BN <= 256, "wgmma N constraint");
@@ -278,19 +281,30 @@ __device__ __forceinline__ void sk_gather(const GemmParams& p, float (&acc)[BN /
   }
 }
 
+// Origin of an M tile in the output raster.  The 128 rows of a tile are a bw x bh x bn box of pixels, all three
+// powers of two (pfd_gemm_f16), so a tile row splits into (x, y, image) with shifts: lbw = log2(bw), lbh = log2(bh).
+struct TileOrigin {
+  int x0, y0, n0, lbw, lbh;
+};
+__device__ __forceinline__ TileOrigin tile_origin(const GemmParams& p, int m_tile) {
+  TileOrigin o;
+  o.x0 = (m_tile % p.tiles_w) * p.bw;
+  o.y0 = ((m_tile / p.tiles_w) % p.tiles_h) * p.bh;
+  o.n0 = (m_tile / (p.tiles_w * p.tiles_h)) * p.bn;
+  o.lbw = __ffs(p.bw) - 1;
+  o.lbh = __ffs(p.bh) - 1;
+  return o;
+}
 // Position of a tile row in the output raster: (x, y, image n) and whether it lies inside the raster.
 struct TileRow {
   int x, y, n;
   bool valid;
 };
-__device__ __forceinline__ TileRow tile_row(const GemmParams& p, int m_tile, int row) {
-  const int tx = m_tile % p.tiles_w;
-  const int ty = (m_tile / p.tiles_w) % p.tiles_h;
-  const int tn = m_tile / (p.tiles_w * p.tiles_h);
+__device__ __forceinline__ TileRow tile_row(const GemmParams& p, const TileOrigin& o, int row) {
   TileRow r;
-  r.x = tx * p.bw + row % p.bw;
-  r.y = ty * p.bh + (row / p.bw) % p.bh;
-  r.n = tn * p.bn + row / (p.bw * p.bh);
+  r.x = o.x0 + (row & (p.bw - 1));
+  r.y = o.y0 + ((row >> o.lbw) & (p.bh - 1));
+  r.n = o.n0 + (row >> (o.lbw + o.lbh));
   r.valid = (r.x < p.W) && (r.y < p.H) && (r.n < p.NB);
   return r;
 }
@@ -306,23 +320,31 @@ __device__ __forceinline__ long long out_col_off(const GemmParams& p, int c) {
 // rows 16 wl + l/4 (+ 8) and, for every 8-column group j, the column pair 8j + 2 (l % 4) (+ 1): acc[4j + {0, 1}] for
 // the first row, acc[4j + {2, 3}] for the second.
 //
+// Bias of a thread's BN / 8 column pairs of tile `tile`.  The consumers issue these loads before the tile's K loop, so
+// their latency lies under the MMAs.  A GEGLU tile is packed [value(BN/2) | gate(BN/2)] in weights and bias alike
+// (pack_geglu), so element j is the value bias of pair j for j < BN / 16 and the gate bias of pair j - BN / 16 after.
+template <int BN>
+__device__ __forceinline__ void gemm_load_bias(const GemmParams& p, int tile, uint32_t (&bias)[BN / 8]) {
+  const int col0 = (tile % p.n_tiles) * BN + 2 * (threadIdx.x & 3);
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) bias[j] = (p.bias && col0 + 8 * j < p.N) ? ldg_h2(p.bias + col0 + 8 * j) : 0u;
+}
+
 // Staged epilogue (every tile with 16-byte addressable output columns, vec_ok, and no split-K): the consumers write
 // the tile's fp16 values into the shared-memory buffer `cbuf` (row pitch C_PITCH) and go on to the next tile; the
 // store warps (gemm_store_tile) add the residual and write the rows to global memory.
-//   * GEGLU (tile packed [value(BN/2) | gate(BN/2)], pack_geglu): fp16(value) * fp16(gelu(fp16(gate))) in columns
-//     [0, BN/2) of the buffer;
+//   * GEGLU: fp16(value) * fp16(gelu(fp16(gate))) in columns [0, BN/2) of the buffer;
 //   * otherwise fp16(act(acc * alpha + bias + row add)).
-// The bias and row-add loads of a block of column groups are all issued before any of them is used.
-template <int BN>
-__device__ __forceinline__ void gemm_stage_tile(const GemmParams& p, const float (&acc)[BN / 2], int cw, int tile,
-                                                uint8_t* cbuf) {
+// The row-add loads of a block of column groups are all issued before any of them is used.
+template <int BN, bool GEGLU>
+__device__ __forceinline__ void gemm_stage_tile(const GemmParams& p, const float (&acc)[BN / 2],
+                                                const uint32_t (&bias)[BN / 8], int cw, int tile, uint8_t* cbuf) {
   constexpr int C_PITCH = GemmCfg<BN>::C_PITCH;
   const int wl = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const int n_tile = tile % p.n_tiles;
-  const int m_tile = tile / p.n_tiles;
-  const bool geglu = (p.act == PFD_ACT_GEGLU);
-  const int n_out = geglu ? p.N / 2 : p.N;
-  const int col_base = n_tile * (geglu ? BN / 2 : BN);
+  const TileOrigin org = tile_origin(p, tile / p.n_tiles);
+  const int n_out = GEGLU ? p.N / 2 : p.N;
+  const int col_base = n_tile * (GEGLU ? BN / 2 : BN);
   const int cq = 2 * (lane & 3);
   int rows[2];
   bool valid[2];
@@ -330,7 +352,7 @@ __device__ __forceinline__ void gemm_stage_tile(const GemmParams& p, const float
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     rows[i] = cw * 64 + wl * 16 + (lane >> 2) + 8 * i;
-    const TileRow r = tile_row(p, m_tile, rows[i]);
+    const TileRow r = tile_row(p, org, rows[i]);
     valid[i] = r.valid;
     rowadd_row[i] = (p.rowadd && r.valid) ? p.rowadd + (long long)r.n * p.rowadd_ld : nullptr;
   }
@@ -338,27 +360,20 @@ __device__ __forceinline__ void gemm_stage_tile(const GemmParams& p, const float
     *reinterpret_cast<__half2*>(cbuf + rows[i] * C_PITCH + c * 2) = h;
   };
   const float alpha = p.alpha;
-  if (geglu) {
-    uint32_t bv[BN / 16], bg[BN / 16];
-#pragma unroll
-    for (int j = 0; j < BN / 16; ++j) {
-      const int c = 8 * j + cq;
-      const bool ld = p.bias && col_base + c < n_out;
-      bv[j] = ld ? ldg_h2(p.bias + (long long)n_tile * BN + c) : 0u;
-      bg[j] = ld ? ldg_h2(p.bias + (long long)n_tile * BN + BN / 2 + c) : 0u;
-    }
+  if (GEGLU) {
 #pragma unroll
     for (int j = 0; j < BN / 16; ++j) {
       const int c = 8 * j + cq;               // value column inside the tile; its gate is column c + BN / 2
       if (col_base + c >= n_out) continue;
+      const uint32_t bv = bias[j], bg = bias[j + BN / 16];
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         if (!valid[i]) continue;
         const float* v = &acc[4 * j + 2 * i];
         const float* g = &acc[4 * (j + BN / 16) + 2 * i];
         // reference: x, gate = proj(x).chunk(2) are fp16 tensors; x * gelu(gate) in fp16 (attention.py:50-51)
-        const __half2 a = __floats2half2_rn(fmaf(v[0], alpha, h2lo(bv[j])), fmaf(v[1], alpha, h2hi(bv[j])));
-        const float2 gf = __half22float2(__floats2half2_rn(fmaf(g[0], alpha, h2lo(bg[j])), fmaf(g[1], alpha, h2hi(bg[j]))));
+        const __half2 a = __floats2half2_rn(fmaf(v[0], alpha, h2lo(bv)), fmaf(v[1], alpha, h2hi(bv)));
+        const float2 gf = __half22float2(__floats2half2_rn(fmaf(g[0], alpha, h2lo(bg)), fmaf(g[1], alpha, h2hi(bg))));
         put(i, c, __hmul2(a, __floats2half2_rn(gelu_sig(gf.x), gelu_sig(gf.y))));
       }
     }
@@ -368,14 +383,12 @@ __device__ __forceinline__ void gemm_stage_tile(const GemmParams& p, const float
   constexpr int JB = (BN / 8) % 8 == 0 ? 8 : 4;   // column groups per block of loads
 #pragma unroll
   for (int j0 = 0; j0 < BN / 8; j0 += JB) {
-    uint32_t bb[JB], ra[2][JB];
+    uint32_t ra[2][JB];
 #pragma unroll
     for (int jj = 0; jj < JB; ++jj) {
       const int col = col_base + 8 * (j0 + jj) + cq;
-      const bool in = col < n_out;
-      bb[jj] = (p.bias && in) ? ldg_h2(p.bias + col) : 0u;
 #pragma unroll
-      for (int i = 0; i < 2; ++i) ra[i][jj] = (rowadd_row[i] && in) ? ldg_h2(rowadd_row[i] + col) : 0u;
+      for (int i = 0; i < 2; ++i) ra[i][jj] = (rowadd_row[i] && col < n_out) ? ldg_h2(rowadd_row[i] + col) : 0u;
     }
 #pragma unroll
     for (int jj = 0; jj < JB; ++jj) {
@@ -384,8 +397,8 @@ __device__ __forceinline__ void gemm_stage_tile(const GemmParams& p, const float
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         if (!valid[i]) continue;
-        float v0 = fmaf(acc[4 * j + 2 * i], alpha, h2lo(bb[jj]));
-        float v1 = fmaf(acc[4 * j + 2 * i + 1], alpha, h2hi(bb[jj]));
+        float v0 = fmaf(acc[4 * j + 2 * i], alpha, h2lo(bias[j]));
+        float v1 = fmaf(acc[4 * j + 2 * i + 1], alpha, h2hi(bias[j]));
         if (rowadd_row[i]) {
           // per-image row add (time embedding): (conv + bias) + emb -> act, the reference's order
           v0 += h2lo(ra[i][jj]);
@@ -402,67 +415,87 @@ __device__ __forceinline__ void gemm_stage_tile(const GemmParams& p, const float
 }
 
 // Store warps (warps 1-3 of warpgroup 0): write one staged tile from `cbuf` to its output rows in 16-byte chunks and
-// add the residual in fp16 - the reference's `x + f(h)` on fp16 tensors.  A quarter-warp reads 128 contiguous bytes
-// of the buffer.  The output row offsets are computed first (`rowoff`, one of two buffers used by alternate tiles);
-// then each thread issues the residual loads of STORE_BATCH chunks before any of their stores.  The first batch is
-// loaded before waiting for the consumers to fill the buffer (`c_full`, phase `parity`).
-template <int BN>
+// add the residual in fp16 - the reference's `x + f(h)` on fp16 tensors.  A row has CPR chunks, a compile-time number,
+// and a thread keeps ONE chunk column for the whole tile: CPR threads share a row, a pass covers 96 / CPR rows, and the
+// 96 % CPR threads left over idle (16 of 96 at BN = 160, 6 at its GEGLU half).  So the column offset - with the head
+// split's division - is computed once per tile, and the rows of a thread advance by a constant step.  When the tile
+// is 128 consecutive pixels of one raster line (bw = 128: every Linear), a row's offset is the tile's plus row * so_x;
+// other tiles (convolutions) look it up in `rowoff`, filled first (one of two buffers used by alternate tiles).
+// Each thread issues the residual loads of STORE_BATCH passes before any of their stores; the first batch is loaded
+// before waiting for the consumers to fill the buffer (`c_full`, phase `parity`).
+template <int BN, bool GEGLU>
 __device__ __forceinline__ void gemm_store_tile(const GemmParams& p, int tile, const uint8_t* cbuf, long long* rowoff,
                                                 uint32_t c_full, uint32_t parity) {
   constexpr int C_PITCH = GemmCfg<BN>::C_PITCH;
   constexpr int STORE_BATCH = GemmCfg<BN>::STORE_BATCH;
+  constexpr int CPR = (GEGLU ? BN / 2 : BN) / 8;      // 16-byte chunks per tile row
+  constexpr int RPP = STORE_THREADS / CPR;            // rows per pass
+  constexpr int NPASS = (BM + RPP - 1) / RPP;
   const int t = threadIdx.x - 32;
   const int n_tile = tile % p.n_tiles;
-  const int m_tile = tile / p.n_tiles;
+  const TileOrigin org = tile_origin(p, tile / p.n_tiles);
+  const bool line_tile = p.bw == BM;    // bh = bn = 1: the tile lies on raster line y0 of image n0, both in the raster
+  if (!line_tile) {
 #pragma unroll 1
-  for (int row = t; row < BM; row += STORE_THREADS) {
-    const TileRow r = tile_row(p, m_tile, row);
-    rowoff[row] = r.valid ? out_row_off(p, r) : -1;
+    for (int row = t; row < BM; row += STORE_THREADS) {
+      const TileRow r = tile_row(p, org, row);
+      rowoff[row] = r.valid ? out_row_off(p, r) : -1;
+    }
+    asm volatile("bar.sync 2, %0;" ::"n"(STORE_THREADS) : "memory");
   }
-  asm volatile("bar.sync 2, %0;" ::"n"(STORE_THREADS) : "memory");
-  const bool geglu = (p.act == PFD_ACT_GEGLU);
-  const int cpr = (geglu ? BN / 2 : BN) / 8;          // 16-byte chunks per tile row
-  const int col_base = n_tile * cpr * 8;
-  const int n_out = geglu ? p.N / 2 : p.N;
-  const bool add_res = p.residual && !geglu;
-  const int total = BM * cpr;
-  long long off[STORE_BATCH];
-  int soff[STORE_BATCH];
-  uint4 res[STORE_BATCH];
-  auto load_batch = [&](int i0) {
+  const int ch = t % CPR, r0 = t / CPR;
+  const int col = n_tile * CPR * 8 + 8 * ch;
+  const bool col_ok = r0 < RPP && col < (GEGLU ? p.N / 2 : p.N);
+  const long long col_off = out_col_off(p, col);
+  const bool add_res = p.residual && !GEGLU;
+  const uint8_t* const src = cbuf + r0 * C_PITCH + ch * 16;
+
+  // row_off(row): element offset of (row, this thread's chunk) in the output, or -1 outside the raster.  It is cheap
+  // enough to be evaluated again at the store, which keeps the offsets of a batch out of the registers.
+  auto store_rows = [&](auto row_off) {
+    uint4 res[STORE_BATCH];
+    auto load_batch = [&](int pass0) {
 #pragma unroll
-    for (int b = 0; b < STORE_BATCH; ++b) {
-      const int idx = i0 + b * STORE_THREADS;
-      off[b] = -1;
-      if (idx < total) {
-        const int row = idx / cpr, ch = idx - row * cpr;
-        const int col = col_base + 8 * ch;
-        const long long ro = rowoff[row];
-        soff[b] = row * C_PITCH + ch * 16;
-        if (ro >= 0 && col < n_out) {
-          off[b] = ro + out_col_off(p, col);
-          if (add_res) res[b] = __ldg(reinterpret_cast<const uint4*>(p.residual + off[b]));
-        }
+      for (int b = 0; b < STORE_BATCH; ++b) {
+        const int row = r0 + (pass0 + b) * RPP;
+        const long long off = (col_ok && row < BM) ? row_off(row) : -1;
+        if (off >= 0) res[b] = __ldg(reinterpret_cast<const uint4*>(p.residual + off));
       }
+    };
+    if (add_res) load_batch(0);
+    mbar_wait(c_full, parity);
+#pragma unroll 1
+    for (int pass0 = 0; pass0 < NPASS; pass0 += STORE_BATCH) {
+#pragma unroll
+      for (int b = 0; b < STORE_BATCH; ++b) {
+        const int row = r0 + (pass0 + b) * RPP;
+        const long long off = (col_ok && row < BM) ? row_off(row) : -1;
+        if (off < 0) continue;
+        uint4 v = *reinterpret_cast<const uint4*>(src + (pass0 + b) * (RPP * C_PITCH));
+        if (add_res) {
+          __half2* h = reinterpret_cast<__half2*>(&v);
+          const __half2* r = reinterpret_cast<const __half2*>(&res[b]);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) h[k] = __hadd2(h[k], r[k]);
+        }
+        *reinterpret_cast<uint4*>(p.out + off) = v;
+      }
+      if (add_res && pass0 + STORE_BATCH < NPASS) load_batch(pass0 + STORE_BATCH);
     }
   };
-  load_batch(t);
-  mbar_wait(c_full, parity);
-#pragma unroll 1
-  for (int i0 = t; i0 < total; i0 += STORE_THREADS * STORE_BATCH) {
-#pragma unroll
-    for (int b = 0; b < STORE_BATCH; ++b) {
-      if (off[b] < 0) continue;
-      uint4 v = *reinterpret_cast<const uint4*>(cbuf + soff[b]);
-      if (add_res) {
-        __half2* h = reinterpret_cast<__half2*>(&v);
-        const __half2* r = reinterpret_cast<const __half2*>(&res[b]);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) h[k] = __hadd2(h[k], r[k]);
-      }
-      *reinterpret_cast<uint4*>(p.out + off[b]) = v;
-    }
-    if (i0 + STORE_THREADS * STORE_BATCH < total) load_batch(i0 + STORE_THREADS * STORE_BATCH);
+
+  if (line_tile) {
+    const int rows_in = p.W - org.x0;
+    TileRow first;
+    first.x = org.x0; first.y = org.y0; first.n = org.n0;
+    const long long base = out_row_off(p, first) + col_off;
+    const long long so_x = p.so_x;
+    store_rows([&](int row) { return row < rows_in ? base + row * so_x : -1ll; });
+  } else {
+    store_rows([&](int row) {
+      const long long ro = rowoff[row];
+      return ro >= 0 ? ro + col_off : -1ll;
+    });
   }
 }
 
@@ -475,6 +508,7 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const float (
   const int wl = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
   const int n_tile = tile % p.n_tiles;
   const int m_tile = tile / p.n_tiles;
+  const TileOrigin org = tile_origin(p, m_tile);
   const bool geglu = (p.act == PFD_ACT_GEGLU);
   const int n_out = geglu ? p.N / 2 : p.N;
   const int col_base = n_tile * (geglu ? BN / 2 : BN);
@@ -487,7 +521,7 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const float (
   for (int i = 0; i < 2; ++i) {
     const int row = cw * 64 + wl * 16 + (lane >> 2) + 8 * i;
     rows[i] = row;
-    const TileRow r = tile_row(p, m_tile, row);
+    const TileRow r = tile_row(p, org, row);
     valid[i] = r.valid;
     row_off[i] = out_row_off(p, r);
     rowadd_row[i] = (p.rowadd && valid[i]) ? p.rowadd + (long long)r.n * p.rowadd_ld : nullptr;
@@ -628,7 +662,8 @@ gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
       WorkItem w;
       for (int wi = 0; gemm_work<SK>(p, wi, total_tiles, w); ++wi) {
         if (SK && w.mode == 1) continue;
-        gemm_store_tile<BN>(p, w.tile, cbuf, rowoff + (c_phase ? BM : 0), c_full, c_phase);
+        if (p.act == PFD_ACT_GEGLU) gemm_store_tile<BN, true>(p, w.tile, cbuf, rowoff + (c_phase ? BM : 0), c_full, c_phase);
+        else gemm_store_tile<BN, false>(p, w.tile, cbuf, rowoff + (c_phase ? BM : 0), c_full, c_phase);
         __syncwarp();
         if ((threadIdx.x & 31) == 0) mbar_arrive(c_empty);
         c_phase ^= 1u;
@@ -683,6 +718,8 @@ gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
     WorkItem w;
     for (int wi = 0; gemm_work<SK>(p, wi, total_tiles, w); ++wi) {
       const int nkb = w.kb1 - w.kb0;
+      uint32_t bias[BN / 8];
+      if (Cfg::BIAS_EARLY && staged) gemm_load_bias<BN>(p, w.tile, bias);
       int prev = -1;
       for (int kb = 0; kb < nkb; ++kb) {
         mbar_wait(full_bar(stage), phase);
@@ -710,8 +747,10 @@ gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
       }
       if (SK && w.mode == 2) sk_gather<BN>(p, acc, w.tile - p.sk_dp_tiles);
       if (staged) {
+        if (!Cfg::BIAS_EARLY) gemm_load_bias<BN>(p, w.tile, bias);
         mbar_wait(c_empty, c_phase ^ 1u);   // the store warps have read the previous tile out of the buffer
-        gemm_stage_tile<BN>(p, acc, cw, w.tile, cbuf);
+        if (p.act == PFD_ACT_GEGLU) gemm_stage_tile<BN, true>(p, acc, bias, cw, w.tile, cbuf);
+        else gemm_stage_tile<BN, false>(p, acc, bias, cw, w.tile, cbuf);
         __syncwarp();
         if (arrive_lane) mbar_arrive(c_full);
         c_phase ^= 1u;

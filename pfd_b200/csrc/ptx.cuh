@@ -84,21 +84,6 @@ __device__ __forceinline__ void tma_load_3d(uint32_t smem_dst, const void* tmap,
       : "memory");
 }
 
-// TMA store (shared -> global, bulk async-group completion): the source tile must have been made visible to the
-// async proxy (fence.proxy.async after the generic-proxy writes) before the issuing thread executes this.
-__device__ __forceinline__ void tma_store_4d(const void* tmap, uint32_t smem_src, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
-      :
-      : "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_src), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// all bulk groups of this thread have finished READING their shared-memory source (it may be overwritten)
-__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-// all bulk groups of this thread are complete (global writes performed)
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
 // ---------------------------------------------------------------- wgmma
 // K-major, 128-byte-swizzled operand tile (rows of 64 fp16 = 128 B, 8-row atoms 1024 B apart, tile base 1024-B
 // aligned).  wgmma matrix descriptor: start>>4 [0,14), LBO>>4 [16,30) (unused for swizzled K-major: 1),
