@@ -365,6 +365,45 @@ PFD_API int pfd_scribble_blur_u8(const uint8_t* z, int32_t B, int32_t H, int32_t
 PFD_API int pfd_scribble_xdog_f32(const void* x, int32_t src_is_f32, int32_t B, int32_t H, int32_t W, int32_t threshold,
                                   float* out, void* stream);
 
+/*
+ * PiDiNet, the default method of ControlNet.preprocess(type='scribble') (controlnet.py:465-472 ->
+ * controlnet_annotator/pidinet/__init__.py:67-96 around pidinet() of pidinet/model.py:441-666: 'carv4', 60 channels,
+ * dil=24, sa=True).  The input step (exact u8 levels; the BGR flip and the / 255 are folded into the weights) is
+ * pfd_hed_input_f16 + im2col + the init block's GEMM; the trunk's 1x1 convs run on pfd_gemm_f16.  The pixel-difference weights are converted to plain
+ * depthwise kernels when they are packed.  All five are asynchronous on `stream` and graph-capturable, and each output
+ * pixel depends on its own image only.
+ *
+ * pfd_pidinet_dw_f16: depthwise conv1 of a PDC block (model.py:450,457-458): x [B,Hin,Win,C] fp16 (C % 8 == 0,
+ *   16-byte aligned), w fp32 [ks*ks][C] (ks 3 or 5, zero padding ks/2) -> out = relu(conv) fp16 [B,h,w,C].  pool != 0
+ *   (ks 3 only): the conv input is the 2x2 stride-2 max-pool of x (model.py:455-456, floor), also written to pooled
+ *   [B,h,w,C] with h = Hin/2, w = Win/2.
+ * pfd_pidinet_reduce_f16: CDCM's relu + conv1 (model.py:419-420): x [P,C] fp16 (C % 8 == 0, C <= 512) -> m [P,24] fp16
+ *   = relu(x) . w + b; w: device fp32 [C][24], b: device fp32 [24].
+ * pfd_pidinet_cdcm_f16: CDCM's conv2_1..conv2_4 summed (model.py:421-425): m [B,h,w,24] fp16 -> u [B,h,w,24] fp32 =
+ *   sum over dilation d in 5,7,9,11 of the 3x3 conv with dilation d and zero padding d, on the tensor cores.  wpk: the
+ *   four weights [24,24,3,3] arranged as mma.m16n8k16 B fragments: [54 k16 steps][3 n-tiles][32 lanes][4 halves],
+ *   where K runs over (dilation, ky, kx, channel) and a lane (g = lane/4, t = lane%4) of n-tile j holds output
+ *   channel 8j+g at K offsets 2t, 2t+1, 2t+8, 2t+9 of the step.
+ * pfd_pidinet_side_f32: CSAM then MapReduce of one stage (model.py:395-401, 437-438, 616, 626): u [B,h,w,24] fp32 ->
+ *   side [B,h,w] fp32 = a * (mr_w . u) + mr_b with a = sigmoid(conv3x3_pad1(conv1x1_4(relu(u)) + b1)); params: device
+ *   fp32 [PFD_PIDINET_SIDE_PARAMS] = conv1 w [4][24], conv1 b [4], conv2 w [4][9], MapReduce w [24], MapReduce b [1].
+ * pfd_pidinet_fuse_f32: model.py:626-645 and pidinet/__init__.py:88-96 for four fp32 side maps [B,h_k,w_k] (host
+ *   array of device pointers and sizes, h_k <= H, w_k <= W): F.interpolate(bilinear, align_corners=False) to H x W,
+ *   classifier cls[0..3] . e + cls[4] (device fp32 [5]), sigmoid, trunc(clip(edge*255, 0, 255)) / 255 -> float32
+ *   [B,3,H,W] with three equal channels.
+ */
+#define PFD_PIDINET_SIDE_PARAMS 161
+PFD_API int pfd_pidinet_dw_f16(const void* x, int32_t B, int32_t Hin, int32_t Win, int32_t C, int32_t ks, int32_t pool,
+                               const float* w, void* out, void* pooled, void* stream);
+PFD_API int pfd_pidinet_reduce_f16(const void* x, int64_t P, int32_t C, const float* w, const float* b, void* m,
+                                   void* stream);
+PFD_API int pfd_pidinet_cdcm_f16(const void* m, int32_t B, int32_t h, int32_t w, const void* wpk, float* u,
+                                 void* stream);
+PFD_API int pfd_pidinet_side_f32(const float* u, int32_t B, int32_t h, int32_t w, const float* params, float* side,
+                                 void* stream);
+PFD_API int pfd_pidinet_fuse_f32(const float* const* sides, const int32_t* side_h, const int32_t* side_w, int32_t B,
+                                 int32_t H, int32_t W, const float* cls, float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -33,9 +33,12 @@ EXPORTS = [
     "pfd_hed_input_f16", "pfd_hed_pool_side_f16", "pfd_hed_fuse_f32",
     "pfd_timestep_embedding_ft_f16", "pfd_ksampler_step_f32", "pfd_ksampler_begin_step", "pfd_randn_f16",
     "pfd_scribble_hed_f32", "pfd_scribble_blur_u8", "pfd_scribble_xdog_f32",
+    "pfd_pidinet_dw_f16", "pfd_pidinet_reduce_f16", "pfd_pidinet_cdcm_f16", "pfd_pidinet_side_f32",
+    "pfd_pidinet_fuse_f32",
 ]
 PFD_KSAMPLER_NCOEF = 6
 PFD_HED_MAX_SIDES = 5
+PFD_PIDINET_SIDE_PARAMS = 161
 
 
 class GemmDesc(ctypes.Structure):
@@ -145,6 +148,13 @@ def load() -> ctypes.CDLL:
     lib.pfd_scribble_hed_f32.argtypes = [c_void_p, c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]
     lib.pfd_scribble_blur_u8.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]
     lib.pfd_scribble_xdog_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]
+    lib.pfd_pidinet_dw_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p,
+                                       c_void_p, c_void_p, c_void_p]
+    lib.pfd_pidinet_reduce_f16.argtypes = [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]
+    lib.pfd_pidinet_cdcm_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]
+    lib.pfd_pidinet_side_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]
+    lib.pfd_pidinet_fuse_f32.argtypes = [POINTER(c_void_p), POINTER(c_int32), POINTER(c_int32), c_int32, c_int32,
+                                         c_int32, c_void_p, c_void_p, c_void_p]
     for name in EXPORTS:
         if hasattr(lib, name) and name not in ("pfd_version", "pfd_last_error", "pfd_launch_count",
                                                "pfd_canny_workspace_bytes"):
@@ -698,6 +708,89 @@ def scribble_xdog(x: torch.Tensor, threshold: int = 32) -> torch.Tensor:
     out = torch.empty((B, 3, H, W), device=x.device, dtype=torch.float32)
     _check(load().pfd_scribble_xdog_f32(x.data_ptr(), int(x.dtype == torch.float32), B, H, W, int(threshold),
                                         out.data_ptr(), stream_ptr()), "pfd_scribble_xdog_f32")
+    return out
+
+
+def pidinet_dw(x: torch.Tensor, w: torch.Tensor, pool: bool = False):
+    """Depthwise conv1 of a PiDiNet block: channel-last x [B,H,W,C] fp16, w CUDA fp32 [ks*ks, C] (ks 3 or 5) ->
+    relu(conv) [B,h,w,C] fp16, and with pool=True (ks 3) the 2x2 max-pooled input it convolved, [B,H/2,W/2,C]
+    (pfd_pidinet_dw_f16)."""
+    _chk16(x, "pidinet_dw x")
+    _chk32(w, "pidinet_dw w")
+    x = x.contiguous()
+    B, H, W, C = x.shape
+    ks = {9: 3, 25: 5}.get(w.shape[0], 0)
+    if w.dim() != 2 or w.shape[1] != C or not ks:
+        raise RuntimeError(f"pidinet_dw: weights {tuple(w.shape)} do not fit C={C}")
+    h, wd = (H // 2, W // 2) if pool else (H, W)
+    out = torch.empty((B, h, wd, C), device=x.device, dtype=torch.float16)
+    pooled = torch.empty_like(out) if pool else None
+    _check(load().pfd_pidinet_dw_f16(x.data_ptr(), B, H, W, C, ks, int(pool), w.data_ptr(), out.data_ptr(), _p(pooled),
+                                     stream_ptr()), "pfd_pidinet_dw_f16")
+    return (out, pooled) if pool else out
+
+
+def pidinet_reduce(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """CDCM's relu + 1x1 conv to 24 channels: x [B,h,w,C] fp16, w CUDA fp32 [C, 24], b [24] -> [B,h,w,24] fp16
+    (pfd_pidinet_reduce_f16)."""
+    _chk16(x, "pidinet_reduce x")
+    _chk32(w, "pidinet_reduce w")
+    _chk32(b, "pidinet_reduce b")
+    x = x.contiguous()
+    B, h, wd, C = x.shape
+    if tuple(w.shape) != (C, 24) or b.numel() != 24:
+        raise RuntimeError(f"pidinet_reduce: weights {tuple(w.shape)} / bias {tuple(b.shape)} do not fit C={C}")
+    m = torch.empty((B, h, wd, 24), device=x.device, dtype=torch.float16)
+    _check(load().pfd_pidinet_reduce_f16(x.data_ptr(), B * h * wd, C, w.data_ptr(), b.data_ptr(), m.data_ptr(),
+                                         stream_ptr()), "pfd_pidinet_reduce_f16")
+    return m
+
+
+def pidinet_cdcm(m: torch.Tensor, wpk: torch.Tensor) -> torch.Tensor:
+    """Sum of CDCM's four dilated 3x3 convs: m [B,h,w,24] fp16, wpk the packed fragments (pidinet.pack_cdcm) ->
+    [B,h,w,24] fp32 (pfd_pidinet_cdcm_f16)."""
+    _chk16(m, "pidinet_cdcm m")
+    _chk16(wpk, "pidinet_cdcm wpk")
+    m = m.contiguous()
+    B, h, w, C = m.shape
+    if C != 24 or wpk.numel() != 54 * 3 * 32 * 4:
+        raise RuntimeError(f"pidinet_cdcm: m {tuple(m.shape)} / packed weights {wpk.numel()} do not fit")
+    u = torch.empty((B, h, w, 24), device=m.device, dtype=torch.float32)
+    _check(load().pfd_pidinet_cdcm_f16(m.data_ptr(), B, h, w, wpk.data_ptr(), u.data_ptr(), stream_ptr()),
+           "pfd_pidinet_cdcm_f16")
+    return u
+
+
+def pidinet_side(u: torch.Tensor, params: torch.Tensor) -> torch.Tensor:
+    """CSAM + MapReduce of a stage: u [B,h,w,24] fp32 -> side map [B,h,w] fp32 (pfd_pidinet_side_f32)."""
+    _chk32(u, "pidinet_side u")
+    _chk32(params, "pidinet_side params")
+    B, h, w, C = u.shape
+    if C != 24 or params.numel() != PFD_PIDINET_SIDE_PARAMS:
+        raise RuntimeError(f"pidinet_side: u {tuple(u.shape)} / params {params.numel()} do not fit")
+    side = torch.empty((B, h, w), device=u.device, dtype=torch.float32)
+    _check(load().pfd_pidinet_side_f32(u.data_ptr(), B, h, w, params.data_ptr(), side.data_ptr(), stream_ptr()),
+           "pfd_pidinet_side_f32")
+    return side
+
+
+def pidinet_fuse(sides: Sequence[torch.Tensor], cls: torch.Tensor, H: int, W: int) -> torch.Tensor:
+    """Four fp32 side maps [B,h_k,w_k] -> float32 [B,3,H,W] levels / 255 (pfd_pidinet_fuse_f32).  cls: CUDA fp32 [5]
+    = classifier weights, bias."""
+    if len(sides) != 4:
+        raise RuntimeError(f"pidinet_fuse: {len(sides)} side maps (4 expected)")
+    _chk32(cls, "pidinet_fuse cls")
+    B = sides[0].shape[0]
+    for s in sides:
+        _chk32(s, "pidinet_fuse side map")
+        if s.dim() != 3 or s.shape[0] != B:
+            raise RuntimeError(f"pidinet_fuse: side maps must be [B,h,w] with B={B}, got {tuple(s.shape)}")
+    out = torch.empty((B, 3, H, W), device=sides[0].device, dtype=torch.float32)
+    ptrs = (c_void_p * 4)(*[s.data_ptr() for s in sides])
+    hs = (c_int32 * 4)(*[s.shape[1] for s in sides])
+    ws = (c_int32 * 4)(*[s.shape[2] for s in sides])
+    _check(load().pfd_pidinet_fuse_f32(ptrs, hs, ws, B, H, W, cls.data_ptr(), out.data_ptr(), stream_ptr()),
+           "pfd_pidinet_fuse_f32")
     return out
 
 

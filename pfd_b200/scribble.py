@@ -6,7 +6,10 @@
     method='xdog'    difference of float32 Gaussians (sigma 0.5 and 5) of the uint8 RGB image, minimum over the
                      channels, uint8 truncation, edge where uint8(2 * uint8(255 - dog)) > threshold
                                                                                         (pfd_scribble_xdog_f32)
-    method='pidinet' (the reference's default) needs the PiDiNet network, which pfd_b200 does not provide.
+    method='pidinet' (the reference's default) the PiDiNet network (pidinet.py), then the same make_scribble kernels
+                     on its uint8 levels                                                (pfd_scribble_hed_f32)
+                     PiDiNet needs its weights: pidinet.load_pidinet / set_network, or table5_pidinet.pth at
+                     pidinet.DEFAULT_PATH.  Without them this method raises NotImplementedError, as before.
 
 The reference's xdog branch cannot run as written (it passes device= to a one-argument function and would return nine
 channels); this is what its lines compute, as three equal channels like every other type.  The product
@@ -33,8 +36,12 @@ def preprocess_scribble(x: torch.Tensor, method: str = "pidinet", threshold=32) 
         t = min(max(math.floor(threshold), -1), 255)
         return nv.scribble_xdog(x, t)
     if method == "pidinet":
-        raise NotImplementedError("scribble method 'pidinet' needs the PiDiNet network, which pfd_b200 does not "
-                                  "provide: use method='hed' or method='xdog', or feed a ready control map "
-                                  "(do_preprocess=False)")
-    raise ValueError(f"unknown scribble method {method!r} (pfd_b200 runs 'hed' and 'xdog'; 'pidinet' is not "
-                     "implemented)")
+        from . import pidinet
+        if not pidinet.available():
+            raise NotImplementedError(
+                "scribble method 'pidinet' needs the PiDiNet weights, which are not installed: use method='hed' or "
+                f"method='xdog', put table5_pidinet.pth at {pidinet.DEFAULT_PATH}, call "
+                "pfd_b200.pidinet.load_pidinet(path) or pfd_b200.pidinet.set_network(net), or feed a ready control "
+                "map (do_preprocess=False)")
+        return nv.scribble_hed(pidinet.preprocess_pidinet(x))
+    raise ValueError(f"unknown scribble method {method!r} (pfd_b200 runs 'pidinet', 'hed' and 'xdog')")
