@@ -47,14 +47,11 @@ PFD_API const char* pfd_last_error(void);
 PFD_API int64_t pfd_launch_count(void);
 /* Run-time tuning switches, so that variants can be A/B-timed inside one process (tools/ab_unet.py); name == NULL
  * resets all of them to the built-in defaults.  Unknown names are stored and ignored.  Known names (default):
- *   gemm_streamk (0)   stream-K tail of the persistent GEMM (ignored in deterministic mode)
- *   flash_poly_mod (0) exponent path of the attention softmax for d <= 64: 1 = packed-half MUFU, n > 1 = every n-th
- *                      pair on the FMA pipe
  *   deterministic (0)  1 = deterministic mode: with the same build on the same GPU architecture, every output of the
  *                      library is a bitwise function of the sample's own inputs - the same across runs and processes,
  *                      batch compositions (sample i of a batch equals the sample computed alone), GPU counts and SM
  *                      counts.  GroupNorm adds its statistics in a fixed order (no float atomics; chunks sized from
- *                      HW and C only), and the GEMM never splits K and ignores gemm_streamk.  Results stay within
+ *                      HW and C only), and the GEMM never splits K.  Results stay within
  *                      rounding of the default mode but are not bit-equal to it.  The default is 1 when the
  *                      environment variable PFD_DETERMINISTIC=1 is set when the library is loaded; a reset
  *                      (name == NULL) returns to that default.  CUDA graphs captured before the switch keep the
@@ -73,7 +70,7 @@ PFD_API int pfd_set_option(const char* name, int32_t value);
  *
  * Rounding: the sum is accumulated in fp32; acc*alpha + bias + rowadd and the activation are evaluated in fp32 and
  *   rounded to fp16 once, y = fp16(act(...)); the residual is then added in fp16, out = fp16(y + residual) - the
- *   reference's `x + f(h)` on fp16 tensors.  Every path (staged or direct epilogue, split-K finish, stream-K) rounds
+ *   reference's `x + f(h)` on fp16 tensors.  Every path (staged or direct epilogue, split-K finish) rounds
  *   at these two points, so the plan changes only the fp32 summation order of the accumulator.
  *
  * Replaces: torch.nn.functional.conv2d / F.linear / torch.einsum / torch.bmm at

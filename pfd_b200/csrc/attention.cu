@@ -11,8 +11,6 @@
 //                                     operand fragment), B = the V^T block (d rows x 64 keys, K-major) from shared memory.
 //   warp 8     : TMA producer (Q once; K and V^T blocks through 2-stage rings released by the consumer warps).
 //   The row sum l accumulates the fp16-rounded probabilities, the values the PV product actually uses.
-//   Optional exponent paths (flash_poly_mod, d <= 64): packed-half MUFU (1), polynomial on the FMA pipe for every
-//   n-th pair (n > 1).
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -29,40 +27,12 @@ namespace pfd {
 constexpr int FA_BQ = 128;
 constexpr int FA_BKV = 64;
 constexpr int FA_THREADS = 288;       // 2 consumer warpgroups + 1 producer warp
-constexpr int FLASH_POLY_MOD_DEFAULT = 0;
 
 __device__ __forceinline__ float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }
-__device__ __forceinline__ uint32_t ex2_f16x2(uint32_t x) {
-  uint32_t y;
-  asm("ex2.approx.f16x2 %0, %1;" : "=r"(y) : "r"(x));
-  return y;
-}
 __device__ __forceinline__ float fast_exp2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
-}
-
-// 2^t for two logits on the FMA / ALU pipes in packed half2 (the softmax of the d = 40 level is bound by the MUFU pipe:
-// 16 ex2 per clock per SM against 4 * d MMA flops per exponential): Cody-Waite split t = n + f with n = round(t) taken
-// from the mantissa of t + 1536 (ulp 1 in that binade), 2^f on [-0.5, 0.5] by a degree-3 polynomial in fp16 Horner
-// form (max rel. error 7e-4, rms 2.5e-4: the size of the fp16 rounding P gets anyway; tools/fit_exp2.py), and 2^n built
-// from the same mantissa bits as a half whose exponent field is n + 15 (t < -15 -> +0.0, like the flushed MUFU path).
-// 12 issue slots per pair instead of 2 MUFU + 1 F2FP.  Valid for t <= 15.
-__device__ __forceinline__ uint32_t exp2_poly_h2(float t0, float t1) {
-  const __half2 lo = __floats2half2_rn(-15.f, -15.f), magic = __floats2half2_rn(1536.f, 1536.f);
-  const __half2 c3 = __floats2half2_rn(0.05592204f, 0.05592204f), c2 = __floats2half2_rn(0.24264008f, 0.24264008f);
-  const __half2 c1 = __floats2half2_rn(0.69312103f, 0.69312103f), c0 = __floats2half2_rn(0.99992448f, 0.99992448f);
-  const __half2 h = __hmax2(__floats2half2_rn(t0, t1), lo);
-  const __half2 r = __hadd2(h, magic);
-  const __half2 f = __hsub2(h, __hsub2(r, magic));
-  __half2 pz = __hfma2(c3, f, c2);
-  pz = __hfma2(pz, f, c1);
-  pz = __hfma2(pz, f, c0);
-  const uint32_t rb = *reinterpret_cast<const uint32_t*>(&r);
-  const uint32_t sb = ((rb & 0x03ff03ffu) - 0x01f101f1u) << 10;
-  const __half2 o = __hmul2(pz, *reinterpret_cast<const __half2*>(&sb));
-  return *reinterpret_cast<const uint32_t*>(&o);
 }
 
 struct alignas(64) FlashParams {
@@ -89,22 +59,7 @@ __device__ __forceinline__ uint32_t pack_f2h(float a, float b) {
   return *reinterpret_cast<const uint32_t*>(&h);
 }
 
-// PM > 1: every PM-th pair of exponentials of a key block takes the polynomial path (exp2_poly_h2) instead of MUFU;
-// PM = 1: every pair goes through ONE packed-half MUFU op (ex2.approx.f16x2)
-template <int PM>
-__device__ __forceinline__ uint32_t exp2_pair(float t0, float t1, int pair) {
-  if (PM == 1) {
-    // both exponentials in ONE MUFU op on packed halves (t <= 0 rounded to fp16 first: the exponent error is <= 2^-7 for
-    // the smallest terms and <= 2^-11 for the ones that matter - the size of the fp16 rounding of the reference's own
-    // score tensor, attention.py:188)
-    const __half2 th = __floats2half2_rn(t0, t1);
-    return ex2_f16x2(*reinterpret_cast<const uint32_t*>(&th));
-  }
-  if (PM > 1 && (pair % (PM > 1 ? PM : 2)) == (PM > 1 ? PM : 2) - 1) return exp2_poly_h2(t0, t1);
-  return pack_f2h(fast_exp2(t0), fast_exp2(t1));
-}
-
-template <int DCH, int DP, int PM>
+template <int DCH, int DP>
 __global__ void __launch_bounds__(FA_THREADS, DCH == 1 ? 2 : 1)
 flash_attn_kernel(const __grid_constant__ FlashParams p) {
   using Cfg = FlashCfg<DCH, DP>;
@@ -254,7 +209,7 @@ flash_attn_kernel(const __grid_constant__ FlashParams p) {
       for (int r = 0; r < 4; ++r) {
         const int i = r & 1;                    // row r0 (i = 0) or r0 + 8
         const int idx = 8 * k + 4 * (r >> 1) + 2 * i;
-        const uint32_t h = exp2_pair<PM>(fmaf(s[idx], c2, nm[i]), fmaf(s[idx + 1], c2, nm[i]), 4 * k + r);
+        const uint32_t h = pack_f2h(fast_exp2(fmaf(s[idx], c2, nm[i])), fast_exp2(fmaf(s[idx + 1], c2, nm[i])));
         const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&h));
         l[i] += hf.x + hf.y;
         pa[k][r] = h;
@@ -319,29 +274,18 @@ static int encode4d(CUtensorMap* m, const void* ptr, cuuint64_t inner, cuuint64_
   return 0;
 }
 
-template <int DCH, int DP, int PM>
+template <int DCH, int DP>
 static int launch_flash(const FlashParams& p, dim3 grid, cudaStream_t st) {
   using Cfg = FlashCfg<DCH, DP>;
   static bool done = false;
   if (!done) {
-    cudaError_t e = cudaFuncSetAttribute(flash_attn_kernel<DCH, DP, PM>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(flash_attn_kernel<DCH, DP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          Cfg::SMEM_BYTES);
     if (e != cudaSuccess) return set_error("cudaFuncSetAttribute(flash d<=%d): %s", DP, cudaGetErrorString(e));
     done = true;
   }
-  launch_k(flash_attn_kernel<DCH, DP, PM>, grid, dim3(FA_THREADS), (size_t)Cfg::SMEM_BYTES, st, p);
+  launch_k(flash_attn_kernel<DCH, DP>, grid, dim3(FA_THREADS), (size_t)Cfg::SMEM_BYTES, st, p);
   return check_launch("pfd_flash_attn_f16");
-}
-
-template <int DP>
-static int launch_flash_pm(const FlashParams& p, dim3 grid, cudaStream_t st) {
-  // d <= 64 is MUFU-bound: a share of the exponentials may go to the FMA pipe ("flash_poly_mod": every n-th pair)
-  const int pm = option("flash_poly_mod", FLASH_POLY_MOD_DEFAULT);
-  if (pm == 1) return launch_flash<1, DP, 1>(p, grid, st);
-  if (pm == 2) return launch_flash<1, DP, 2>(p, grid, st);
-  if (pm == 3) return launch_flash<1, DP, 3>(p, grid, st);
-  if (pm == 4) return launch_flash<1, DP, 4>(p, grid, st);
-  return launch_flash<1, DP, 0>(p, grid, st);
 }
 
 }  // namespace pfd
@@ -372,18 +316,18 @@ extern "C" PFD_API int pfd_flash_attn_strided_f16(const void* q, const void* k, 
   p.o_sb = o_sb; p.o_sq = o_sq; p.o_sh = d;
   dim3 grid((Nq + FA_BQ - 1) / FA_BQ, (unsigned)((long long)B * heads));
   switch ((d + 15) / 16) {
-    case 1: return launch_flash_pm<16>(p, grid, st);
-    case 2: return launch_flash_pm<32>(p, grid, st);
-    case 3: return launch_flash_pm<48>(p, grid, st);
-    case 4: return launch_flash_pm<64>(p, grid, st);
-    case 5: return launch_flash<2, 80, 0>(p, grid, st);
-    case 6: return launch_flash<2, 96, 0>(p, grid, st);
-    case 7: return launch_flash<2, 112, 0>(p, grid, st);
-    case 8: return launch_flash<2, 128, 0>(p, grid, st);
-    case 9: return launch_flash<3, 144, 0>(p, grid, st);
-    case 10: return launch_flash<3, 160, 0>(p, grid, st);
-    case 11: return launch_flash<3, 176, 0>(p, grid, st);
-    default: return launch_flash<3, 192, 0>(p, grid, st);
+    case 1: return launch_flash<1, 16>(p, grid, st);
+    case 2: return launch_flash<1, 32>(p, grid, st);
+    case 3: return launch_flash<1, 48>(p, grid, st);
+    case 4: return launch_flash<1, 64>(p, grid, st);
+    case 5: return launch_flash<2, 80>(p, grid, st);
+    case 6: return launch_flash<2, 96>(p, grid, st);
+    case 7: return launch_flash<2, 112>(p, grid, st);
+    case 8: return launch_flash<2, 128>(p, grid, st);
+    case 9: return launch_flash<3, 144>(p, grid, st);
+    case 10: return launch_flash<3, 160>(p, grid, st);
+    case 11: return launch_flash<3, 176>(p, grid, st);
+    default: return launch_flash<3, 192>(p, grid, st);
   }
 }
 

@@ -9,10 +9,9 @@
 // (bias / time-embedding / activation / GEGLU) and write the fp16 tile to a shared-memory staging buffer, then go on
 // to the next tile's K blocks; the store warps add the residual and write the tile to global memory with 16-byte
 // stores while those MMAs run (gemm_stage_tile / gemm_store_tile, barriers c_full / c_empty).  Split-K partials and
-// element-strided outputs keep the direct epilogue from the registers (gemm_epilogue); stream-K contributors hand
-// their fp32 partial tile to the owner, whose epilogue is staged.  The producer runs ahead through a ring of
-// shared-memory stages, so the loads of tile i+1 overlap the epilogue of tile i.  See include/pfd_b200.h
-// (pfd_gemm_f16) for the reference call sites this replaces.
+// element-strided outputs keep the direct epilogue from the registers (gemm_epilogue).  The producer runs ahead
+// through a ring of shared-memory stages, so the loads of tile i+1 overlap the epilogue of tile i.  See
+// include/pfd_b200.h (pfd_gemm_f16) for the reference call sites this replaces.
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -53,11 +52,6 @@ struct alignas(64) GemmParams {
   int splits;        // split-K factor (1 = off); work items = tiles * splits
   int kb_per_split;
   float* ws;         // fp32 partials [splits][m_tiles*128][N] when splits > 1
-  // stream-K tail: tiles < sk_dp_tiles are processed whole, one per CTA per wave; the K blocks of the remaining sk_R
-  // tiles are spread evenly over ALL CTAs (see gemm_work)
-  int sk_dp_tiles, sk_R;
-  float* sk_ws;      // fp32 partial tiles [2 * grid][BN / 8][256 consumer threads][4]
-  int* sk_flags;     // [2 * grid] 0 / 1, reset by the consumer
   float alpha;
   int act;
   const __half* bias;
@@ -86,7 +80,7 @@ struct GemmCfg {
   // Register budgets (setmaxnreg) of the two roles.  The CTA starts with 168 per thread (__launch_bounds__(384, 1)),
   // so 128 PRODUCER_REGS + 256 CONSUMER_REGS = 384 x 168.  The producer warpgroup's budget bounds the store warps'
   // STORE_BATCH (16-byte chunks per thread whose residual loads are in flight at once); the 256-wide tile's consumers
-  // (128 fp32 accumulators) need more than 216 registers with the stream-K gather.
+  // hold 128 fp32 accumulators, so they get the larger budget.
   static constexpr int CONSUMER_REGS = BN >= 256 ? 224 : 208;
   static constexpr int PRODUCER_REGS = BN >= 256 ? 56 : 88;
   static constexpr int STORE_BATCH = BN >= 256 ? 4 : 8;
@@ -164,121 +158,20 @@ __device__ __forceinline__ float h2lo(uint32_t u) { return __low2float(*reinterp
 __device__ __forceinline__ float h2hi(uint32_t u) { return __high2float(*reinterpret_cast<const __half2*>(&u)); }
 __device__ __forceinline__ uint32_t ldg_h2(const __half* p) { return __ldg(reinterpret_cast<const unsigned int*>(p)); }
 
-// One unit of work of a persistent CTA: K blocks [kb0, kb1) of output tile `tile`.
-//   mode 0: the whole contraction of the tile (or, with split-K, slice `slot`) -> normal epilogue
-//   mode 1: stream-K contributor: raw fp32 partial tile -> sk_ws[slot], then sk_flags[slot] = 1
-//   mode 2: stream-K owner (its range ends with the tile's last K block): adds the contributors' partials, normal epilogue
-// Stream-K tail: with T tiles on G CTAs the last wave holds R = T mod G tiles.  Their R * num_kb K blocks are cut into
-// G equal contiguous ranges; a range covers the tail of one tile (processed LAST: this CTA owns that tile if it reaches
-// its end) and possibly the head of the next (processed FIRST: a pure contributor that depends on nobody, so its
-// partial is published early and the owner - the next CTA - rarely waits).
+// One unit of work of a persistent CTA: K blocks [kb0, kb1) of output tile `tile`, the whole contraction of the tile
+// or, with split-K, slice `slot`.
 struct WorkItem {
-  int tile, kb0, kb1, mode, slot;
+  int tile, kb0, kb1, slot;
 };
-__device__ __forceinline__ void sk_range(const GemmParams& p, int c, int G, int& u0, int& u1) {
-  const long long U = (long long)p.sk_R * p.num_kb;
-  u0 = (int)(U * c / G);
-  u1 = (int)(U * (c + 1) / G);
-}
-template <bool SK>
 __device__ __forceinline__ bool gemm_work(const GemmParams& p, int wi, int total_tiles, WorkItem& w) {
   const int G = gridDim.x, c = blockIdx.x;
-  if (!SK || p.sk_R == 0) {
-    const int work = c + wi * G;
-    if (work >= total_tiles * p.splits) return false;
-    w.tile = work % total_tiles;
-    w.slot = work / total_tiles;
-    w.kb0 = w.slot * p.kb_per_split;
-    w.kb1 = min(p.num_kb, w.kb0 + p.kb_per_split);
-    w.mode = 0;
-    return true;
-  }
-  // the stream-K segments come FIRST and the whole tiles after them, so the contributor -> flag -> owner hand-off is
-  // hidden behind the whole tiles of the same CTA and the kernel ends with balanced whole tiles
-  int u0, u1;
-  sk_range(p, c, G, u0, u1);
-  const int KB = p.num_kb;
-  const int t0 = u0 / KB;
-  const int aend = min(u1, (t0 + 1) * KB);
-  const bool has_b = u1 > aend;                        // the range spills into tile t0 + 1
-  const int nseg = (u1 > u0) ? (has_b ? 2 : 1) : 0;
-  if (wi >= nseg) {
-    const int n_dp = p.sk_dp_tiles / G;                // whole waves
-    if (wi - nseg >= n_dp) return false;
-    w.tile = c + (wi - nseg) * G; w.kb0 = 0; w.kb1 = p.num_kb; w.mode = 0; w.slot = 0;
-    return true;
-  }
-  int s0, s1, t;
-  if (wi == 0 && has_b) { s0 = aend; s1 = u1; t = t0 + 1; }
-  else { s0 = u0; s1 = aend; t = t0; }
-  w.tile = p.sk_dp_tiles + t;
-  w.kb0 = s0 - t * KB;
-  w.kb1 = s1 - t * KB;
-  w.mode = (w.kb1 == KB) ? (w.kb0 == 0 ? 0 : 2) : 1;
-  w.slot = 2 * c + ((wi == 0 && has_b) ? 1 : 0);
+  const int work = c + wi * G;
+  if (work >= total_tiles * p.splits) return false;
+  w.tile = work % total_tiles;
+  w.slot = work / total_tiles;
+  w.kb0 = w.slot * p.kb_per_split;
+  w.kb1 = min(p.num_kb, w.kb0 + p.kb_per_split);
   return true;
-}
-
-__device__ __forceinline__ int ld_acquire_gpu(const int* ptr) {
-  int v;
-  asm volatile("ld.acquire.gpu.global.b32 %0, [%1];" : "=r"(v) : "l"(ptr) : "memory");
-  return v;
-}
-__device__ __forceinline__ void st_release_gpu(int* ptr, int v) {
-  asm volatile("st.release.gpu.global.b32 [%0], %1;" ::"l"(ptr), "r"(v) : "memory");
-}
-
-// Stream-K hand-off of the 256 consumer threads (ctid = threadIdx.x - 128).  A partial tile is stored in fragment order,
-// [slot][float4 group v of the thread's BN / 2 accumulators][ctid], so every warp-wide store / load is one contiguous
-// 512-byte request; contributor and owner threads with the same ctid hold the same tile elements.
-template <int BN>
-__device__ __forceinline__ void sk_publish(const GemmParams& p, const float (&acc)[BN / 2], int slot) {
-  const int ctid = threadIdx.x - 128;
-  float4* pw = reinterpret_cast<float4*>(p.sk_ws) + (long long)slot * (BN / 8) * 256 + ctid;
-#pragma unroll
-  for (int v = 0; v < BN / 8; ++v)
-    __stcg(pw + v * 256, make_float4(acc[4 * v], acc[4 * v + 1], acc[4 * v + 2], acc[4 * v + 3]));
-  __threadfence();
-  asm volatile("bar.sync 1, 256;" ::: "memory");          // every consumer thread's partial is written and fenced
-  if (ctid == 0) st_release_gpu(p.sk_flags + slot, 1);
-}
-// Owner of tail tile t (its range starts at K block > 0): the CTAs whose ranges cover the tile's first K blocks are
-// found by a backwards scan (contributor cc used slot 2cc if its range STARTS inside this tile, 2cc + 1 if it spilled
-// over from the previous tile); their partials are added to the accumulators once their flags are set.
-template <int BN>
-__device__ __forceinline__ void sk_gather(const GemmParams& p, float (&acc)[BN / 2], int t) {
-  const int ctid = threadIdx.x - 128;
-  const int G = gridDim.x;
-  const int tstart = t * p.num_kb;
-  int nsrc = 0, src_slot[6];
-  for (int cc = (int)blockIdx.x - 1; cc >= 0 && nsrc < 6; --cc) {
-    int u0, u1;
-    sk_range(p, cc, G, u0, u1);
-    if (u1 <= tstart) break;
-    if (u1 > u0) src_slot[nsrc++] = (u0 >= tstart) ? 2 * cc : 2 * cc + 1;
-  }
-  if (ctid == 0) {
-    for (int j = 0; j < nsrc; ++j) {
-      uint32_t spins = 0;
-      while (ld_acquire_gpu(p.sk_flags + src_slot[j]) == 0) {
-        __nanosleep(64);
-        if (++spins > (1u << 24)) asm volatile("trap;");
-      }
-      p.sk_flags[src_slot[j]] = 0;                       // consumed: ready for the next launch
-    }
-  }
-  asm volatile("bar.sync 1, 256;" ::: "memory");
-  for (int j = 0; j < nsrc; ++j) {
-    const float4* src = reinterpret_cast<const float4*>(p.sk_ws) + (long long)src_slot[j] * (BN / 8) * 256 + ctid;
-#pragma unroll
-    for (int v = 0; v < BN / 8; ++v) {
-      const float4 u = __ldcg(src + v * 256);
-      acc[4 * v] += u.x;
-      acc[4 * v + 1] += u.y;
-      acc[4 * v + 2] += u.z;
-      acc[4 * v + 3] += u.w;
-    }
-  }
 }
 
 // Origin of an M tile in the output raster.  The 128 rows of a tile are a bw x bh x bn box of pixels, all three
@@ -609,9 +502,7 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const float (
   }
 }
 
-// SK = true: stream-K tail enabled (gemm_work / sk_publish / sk_gather); a separate instantiation so the plain kernel
-// carries none of its state.
-template <int BN, bool SK>
+template <int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
   using Cfg = GemmCfg<BN>;
@@ -632,7 +523,7 @@ gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
   const uint32_t c_full = bars + 16u * STAGES, c_empty = c_full + 8u;
 
   const int wg = threadIdx.x >> 7;
-  // staged epilogue for every tile of the launch except stream-K contributors (see gemm_stage_tile)
+  // staged epilogue for every tile of the launch (see gemm_stage_tile)
   const bool staged = p.vec_ok && p.splits == 1;
 
   if (threadIdx.x == 0) {
@@ -660,8 +551,7 @@ gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
     if (threadIdx.x >= 32 && staged) {
       uint32_t c_phase = 0;
       WorkItem w;
-      for (int wi = 0; gemm_work<SK>(p, wi, total_tiles, w); ++wi) {
-        if (SK && w.mode == 1) continue;
+      for (int wi = 0; gemm_work(p, wi, total_tiles, w); ++wi) {
         if (p.act == PFD_ACT_GEGLU) gemm_store_tile<BN, true>(p, w.tile, cbuf, rowoff + (c_phase ? BM : 0), c_full, c_phase);
         else gemm_store_tile<BN, false>(p, w.tile, cbuf, rowoff + (c_phase ? BM : 0), c_full, c_phase);
         __syncwarp();
@@ -672,7 +562,7 @@ gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
       int stage = 0;
       uint32_t phase = 0;
       WorkItem w;
-      for (int wi = 0; gemm_work<SK>(p, wi, total_tiles, w); ++wi) {
+      for (int wi = 0; gemm_work(p, wi, total_tiles, w); ++wi) {
         const int tile = w.tile, kb_begin = w.kb0, kb_end = w.kb1;
         const int n_tile = tile % p.n_tiles;
         const int m_tile = tile / p.n_tiles;
@@ -716,7 +606,7 @@ gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
     uint32_t phase = 0, c_phase = 0;
     float acc[BN / 2];
     WorkItem w;
-    for (int wi = 0; gemm_work<SK>(p, wi, total_tiles, w); ++wi) {
+    for (int wi = 0; gemm_work(p, wi, total_tiles, w); ++wi) {
       const int nkb = w.kb1 - w.kb0;
       uint32_t bias[BN / 8];
       if (Cfg::BIAS_EARLY && staged) gemm_load_bias<BN>(p, w.tile, bias);
@@ -741,11 +631,6 @@ gemm_wgmma_kernel(const __grid_constant__ GemmParams p) {
       }
       wgmma_wait<0>();
       if (prev >= 0 && arrive_lane) mbar_arrive(empty_bar(prev));
-      if (SK && w.mode == 1) {
-        sk_publish<BN>(p, acc, w.slot);
-        continue;
-      }
-      if (SK && w.mode == 2) sk_gather<BN>(p, acc, w.tile - p.sk_dp_tiles);
       if (staged) {
         if (!Cfg::BIAS_EARLY) gemm_load_bias<BN>(p, w.tile, bias);
         mbar_wait(c_empty, c_phase ^ 1u);   // the store warps have read the previous tile out of the buffer
@@ -838,8 +723,9 @@ splitk_finish_kernel(const __grid_constant__ GemmParams p) {
 }
 
 // ------------------------------------------------------------------------------------------ host
-constexpr size_t SPLITK_WS_BYTES = 64ull << 20;
-constexpr size_t SK_FLAG_BYTES = 4096;          // stream-K flags live at the end of the workspace
+// Size of the split-K workspace, which also bounds the partials of a split-K plan.  It decides which shapes are split
+// and so the bits of their results: keep it at 64 MiB - 4 KiB.
+constexpr size_t SPLITK_WS_BYTES = (64ull << 20) - 4096;
 // One fp32 split-K workspace per DEVICE, allocated by the first pfd_gemm_f16 call on that device that is not
 // inside a stream capture (cudaMalloc is illegal while capturing) - i.e. in the eager warm-up pass that every
 // graph-captured path of this package runs first - and then shared by the eager and the captured launches, so
@@ -863,13 +749,6 @@ static float* splitk_workspace(cudaStream_t st) {
   float* pnew = nullptr;
   if (cudaMalloc(&pnew, SPLITK_WS_BYTES) != cudaSuccess) {
     (void)cudaGetLastError();
-    return nullptr;
-  }
-  // the last SK_FLAG_BYTES hold the stream-K ready flags: zero once, every consumer resets the flags it has read
-  if (cudaMemset(reinterpret_cast<char*>(pnew) + SPLITK_WS_BYTES - SK_FLAG_BYTES, 0, SK_FLAG_BYTES) != cudaSuccess ||
-      cudaDeviceSynchronize() != cudaSuccess) {
-    (void)cudaGetLastError();
-    cudaFree(pnew);
     return nullptr;
   }
   ws[dev] = pnew;
@@ -919,43 +798,9 @@ static int encode_map(CUtensorMap* m, const void* ptr, int rank, const cuuint64_
 
 static inline long long cdivll(long long a, long long b) { return (a + b - 1) / b; }
 
-template <int BN, bool SK>
-static int launch_gemm_t(const GemmParams& p, int grid, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
-  static bool attr_done = false;
-  if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, SK>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_BYTES);
-    if (e != cudaSuccess) return set_error("cudaFuncSetAttribute(gemm BN=%d): %s", BN, cudaGetErrorString(e));
-    attr_done = true;
-  }
-  launch_k(gemm_wgmma_kernel<BN, SK>, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, p);
-  return check_launch("pfd_gemm_f16");
-}
-
 template <int BN>
-static int launch_gemm(GemmParams& p, int grid, cudaStream_t stream) {
-  // stream-K tail (see gemm_work), OPT-IN (gemm_streamk = 1): the tiles of the last, partially filled wave are spread
-  // over all SMs by K range; every tile of the tail must be covered by at most 6 contributors.  Correct and
-  // deterministic; it trades the idle SMs of the last wave for a partial-tile hand-off through L2 per tail tile.
-  p.sk_R = 0;
-  p.sk_dp_tiles = 0;
-  // deterministic mode ignores it: the K ranges of a tail tile would depend on the SM count and the tile count
-  if (p.splits == 1 && !deterministic() && option("gemm_streamk", 0)) {
-    const int G = plan_sms();
-    const long long T = (long long)p.tiles_w * p.tiles_h * p.tiles_nb * p.n_tiles;
-    const long long R = T % G, waves = (T + G - 1) / G;
-    float* ws = splitk_workspace(stream);
-    const size_t need = (size_t)2 * G * BM * BN * sizeof(float);
-    if (ws && R > 0 && p.num_kb >= 16 && R * 6 >= G && (size_t)2 * G * sizeof(int) <= SK_FLAG_BYTES &&
-        need <= SPLITK_WS_BYTES - SK_FLAG_BYTES && (double)T / G < 0.95 * (double)waves) {
-      p.sk_dp_tiles = (int)(T - R);
-      p.sk_R = (int)R;
-      p.sk_ws = ws;
-      p.sk_flags = reinterpret_cast<int*>(reinterpret_cast<char*>(ws) + SPLITK_WS_BYTES - SK_FLAG_BYTES);
-      grid = G;
-    }
-  }
+static int launch_gemm(const GemmParams& p, int grid, cudaStream_t stream) {
+  using Cfg = GemmCfg<BN>;
   static int trace = -1;
   if (trace < 0) {
     const char* e = getenv("PFD_GEMM_TRACE");
@@ -963,10 +808,18 @@ static int launch_gemm(GemmParams& p, int grid, cudaStream_t stream) {
   }
   if (trace)   // one line per launch
     fprintf(stderr, "GEMMTRACE M=%lld N=%d K=%d nseg=%d taps=%d stride=%d act=%d bias=%d res=%d rowadd=%d BN=%d "
-            "splits=%d grid=%d batched=%d vec=%d plain=%d sk=%d\n", (long long)p.W * p.H * p.NB, p.N, p.num_kb * BK,
+            "splits=%d grid=%d batched=%d vec=%d plain=%d\n", (long long)p.W * p.H * p.NB, p.N, p.num_kb * BK,
             p.nseg, p.taps[0], p.stride, p.act, p.bias != nullptr, p.residual != nullptr, p.rowadd != nullptr, BN,
-            p.splits, grid, p.b_batched, p.vec_ok, (int)(p.cdiv >= p.N), p.sk_R);
-  return p.sk_R > 0 ? launch_gemm_t<BN, true>(p, grid, stream) : launch_gemm_t<BN, false>(p, grid, stream);
+            p.splits, grid, p.b_batched, p.vec_ok, (int)(p.cdiv >= p.N));
+  static bool attr_done = false;
+  if (!attr_done) {
+    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         Cfg::SMEM_BYTES);
+    if (e != cudaSuccess) return set_error("cudaFuncSetAttribute(gemm BN=%d): %s", BN, cudaGetErrorString(e));
+    attr_done = true;
+  }
+  launch_k(gemm_wgmma_kernel<BN>, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, p);
+  return check_launch("pfd_gemm_f16");
 }
 
 }  // namespace pfd
@@ -1110,7 +963,7 @@ extern "C" PFD_API int pfd_gemm_f16(const pfd_gemm_desc* d) {
       if (splits > 8) splits = 8;
       if (splits > num_kb / 8) splits = num_kb / 8;
       const size_t need = (size_t)splits * (size_t)m_tiles * BM * (size_t)d->N * sizeof(float);
-      if (splits >= 2 && need <= SPLITK_WS_BYTES - SK_FLAG_BYTES) {
+      if (splits >= 2 && need <= SPLITK_WS_BYTES) {
         float* ws = skws;
         if (ws) {
           BNsel = bn_sk;

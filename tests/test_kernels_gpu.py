@@ -123,18 +123,26 @@ def test_gemm_epilogue_rasters(nv, case):
 
 
 @pytest.mark.parametrize("case", ["conv_res_2tiles", "conv_many_waves", "conv_wide_rowadd_silu", "linear_odd_ragged",
-                                  "conv_stride2", "conv_tiny", "conv_skip_segments"])
+                                  "conv_stride2", "conv_tiny", "conv_skip_segments", "conv_l1", "conv_l2_single_wave",
+                                  "conv_l0_res", "linear_bigk_res", "conv_ragged_rowadd_silu"])
 def test_gemm_conv_tilings(nv, case):
     """Long-K convs and Linears against torch fp32: one / many tiles per CTA of the persistent kernel (pipeline phases
     across tiles), N tiles 256 / 160 / 128, an odd number of 128-row tiles, N not a multiple of the tile, stride 2,
-    per-image row add + SiLU, residual, extra 1x1 K segments."""
+    per-image row add + SiLU, residual, extra 1x1 K segments.  The UNet's batch-8 level convs (a partially filled last
+    wave, or a single wave), a K = 5120 Linear with bias + residual, and 7 images with N = 328 (ragged rows and
+    columns)."""
     def run():
         if case == "linear_odd_ragged":
             x, w, r = rnd(640, 1024), rnd(1288, 1024, scale=1024 ** -0.5, seed=1), rnd(640, 1288, seed=3)
             return nv.linear(x, w, None, residual=r), x.float() @ w.float().t() + r.float()
+        if case == "linear_bigk_res":
+            x, w, b, r = rnd(2048, 5120), rnd(1280, 5120, scale=5120 ** -0.5, seed=1), rnd(1280, seed=2), rnd(2048, 1280, seed=3)
+            return nv.linear(x, w, b, residual=r), x.float() @ w.float().t() + b.float() + r.float()
         NB, H, W, C, N = {"conv_res_2tiles": (2, 64, 64, 320, 320), "conv_many_waves": (8, 64, 64, 128, 320),
                           "conv_wide_rowadd_silu": (2, 32, 32, 128, 1280), "conv_stride2": (4, 32, 32, 128, 256),
-                          "conv_tiny": (3, 8, 8, 128, 128), "conv_skip_segments": (2, 32, 32, 64, 160)}[case]
+                          "conv_tiny": (3, 8, 8, 128, 128), "conv_skip_segments": (2, 32, 32, 64, 160),
+                          "conv_l1": (8, 32, 32, 640, 640), "conv_l2_single_wave": (8, 16, 16, 640, 1280),
+                          "conv_l0_res": (8, 64, 64, 320, 320), "conv_ragged_rowadd_silu": (7, 24, 24, 192, 328)}[case]
         x = rnd(NB, H, W, C)
         w4 = rnd(N, C, 3, 3, scale=(9 * C) ** -0.5, seed=1)
         b = rnd(N, seed=2)
@@ -143,7 +151,10 @@ def test_gemm_conv_tilings(nv, case):
         if case == "conv_stride2":
             out = nv.conv3x3(x, wp, b, stride=2)
             ref = F.conv2d(xr, w4.float(), b.float(), stride=2, padding=1)
-        elif case == "conv_wide_rowadd_silu":
+        elif case in ("conv_l1", "conv_l2_single_wave"):
+            out = nv.conv3x3(x, wp, b)
+            ref = F.conv2d(xr, w4.float(), b.float(), padding=1)
+        elif case in ("conv_wide_rowadd_silu", "conv_ragged_rowadd_silu"):
             ra = rnd(NB, N, seed=5)
             out = nv.conv3x3(x, wp, b, rowadd=ra, act=nv.ACT_SILU)
             ref = F.silu(F.conv2d(xr, w4.float(), b.float(), padding=1) + ra.float()[:, :, None, None])
@@ -161,60 +172,6 @@ def test_gemm_conv_tilings(nv, case):
     out, ref = run()
     torch.cuda.synchronize()
     close(out, ref)
-
-
-@pytest.mark.parametrize("case", ["conv_l1", "conv_l2_single_wave", "conv_l0_res", "linear_bigk_res", "conv_ragged_rowadd_silu"])
-def test_gemm_stream_k_tail(nv, case):
-    """Stream-K tail of the persistent GEMM: the tiles of the last, partially filled wave are cut into K ranges over ALL
-    SMs (contributors publish fp32 partial tiles through the workspace + a ready flag, the CTA that reaches the tile's
-    last K block adds them and runs the normal epilogue).  Against torch fp32 and against the plain tiling
-    (gemm_streamk = 0; only the fp32 summation order differs); each case is launched three times and replayed from a
-    CUDA graph, which must give identical bits (the flags are reset by their consumers)."""
-    if case == "linear_bigk_res":
-        x, w, b, r = rnd(2048, 5120), rnd(1280, 5120, scale=5120 ** -0.5, seed=1), rnd(1280, seed=2), rnd(2048, 1280, seed=3)
-        ref = x.float() @ w.float().t() + b.float() + r.float()
-        run = lambda: nv.linear(x, w, b, residual=r)
-    else:
-        NB, H, W, C, N = {"conv_l1": (8, 32, 32, 640, 640), "conv_l2_single_wave": (8, 16, 16, 640, 1280),
-                          "conv_l0_res": (8, 64, 64, 320, 320), "conv_ragged_rowadd_silu": (7, 24, 24, 192, 328)}[case]
-        x = rnd(NB, H, W, C)
-        w4 = rnd(N, C, 3, 3, scale=(9 * C) ** -0.5, seed=1)
-        b = rnd(N, seed=2)
-        wp = w4.permute(0, 2, 3, 1).reshape(N, 9 * C).contiguous()
-        xr = x.float().permute(0, 3, 1, 2)
-        if case == "conv_ragged_rowadd_silu":
-            ra = rnd(NB, N, seed=5)
-            ref = F.silu(F.conv2d(xr, w4.float(), b.float(), padding=1) + ra.float()[:, :, None, None])
-            run = lambda: nv.conv3x3(x, wp, b, rowadd=ra, act=nv.ACT_SILU)
-        elif case == "conv_l0_res":
-            r = rnd(NB, H, W, N, seed=3)
-            ref = F.conv2d(xr, w4.float(), b.float(), padding=1) + r.float().permute(0, 3, 1, 2)
-            run = lambda: nv.conv3x3(x, wp, b, residual=r)
-        else:
-            ref = F.conv2d(xr, w4.float(), b.float(), padding=1)
-            run = lambda: nv.conv3x3(x, wp, b)
-        ref = ref.permute(0, 2, 3, 1)
-    nv.set_env_option(None, None)
-    try:
-        nv.set_env_option("gemm_streamk", 0)
-        out0 = run().clone()
-        nv.set_env_option("gemm_streamk", 1)       # opt-in (measured slower than the plain tiling on the UNet's shapes)
-        outs = [run().clone() for _ in range(3)]
-        torch.cuda.synchronize()
-        g = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(g):
-            og = run()
-        for _ in range(3):
-            g.replay()
-        torch.cuda.synchronize()
-    finally:
-        nv.set_env_option(None, None)
-    close(out0, ref)
-    close(outs[0], ref)
-    assert torch.equal(outs[0], outs[1]) and torch.equal(outs[0], outs[2]) and torch.equal(outs[0], og), "stream-K launches disagree"
-    dmax = (out0.float() - outs[0].float()).abs().max().item()
-    print(f"[stream-K] {case}: max |stream-K - plain tiling| = {dmax:.3e} (ref max {ref.abs().max().item():.2f})")
-    assert dmax <= 4e-3 * max(1.0, ref.abs().max().item())
 
 
 @pytest.mark.parametrize("C", [64, 320])
@@ -442,7 +399,7 @@ def test_flash_attention(nv, B, heads, Nq, Nk, d):
     s = (torch.bmm(qf, kf.transpose(1, 2)).half().float() * scale).half().float()
     ref = torch.bmm(torch.softmax(s, -1), vf).reshape(B, heads, Nq, d).permute(0, 2, 1, 3).reshape(B, Nq, C)
     close(o_unfused, ref, rtol=6e-3, atol=2e-3)
-    # flash path: packed-half2 exp (MUFU.EX2.F16) -> probabilities carry ~2^-11 relative error
+    # flash path: probabilities rounded to fp16 -> ~2^-11 relative error
     close(o_flash, ref, rtol=8e-3, atol=4e-3)
 
 
@@ -500,14 +457,13 @@ def test_flash_attention_fused_qk_swapped_vt(nv, B, heads, N, d):
     close(o, ref, rtol=8e-3, atol=4e-3)
 
 
-@pytest.mark.parametrize("pm", [1, 2, 3, 4])
 @pytest.mark.parametrize("B,heads,Nq,Nk,d,qscale", [(2, 8, 4096, 4096, 40, 1.0), (2, 8, 1024, 148, 40, 1.0),
                                                    (1, 4, 300, 200, 64, 4.0), (1, 2, 128, 77, 8, 1.0)])
-def test_flash_attention_polynomial_exp2(nv, pm, B, heads, Nq, Nk, d, qscale):
-    """flash_poly_mod = n > 1: every n-th pair of exponentials is computed on the FMA pipe (packed-half2 Cody-Waite +
-    degree-3 polynomial) instead of MUFU; n = 1: every pair in one packed-half MUFU op (ex2.approx.f16x2).  Same tolerance as the MUFU path; qscale = 4 makes peaked rows (logit
-    range ~ +-30: exercises the 2^n scaling, the t < -15 flush and the lazy-rescale headroom)."""
-    g = torch.Generator().manual_seed(pm * 100 + Nq)
+def test_flash_attention_peaked_rows(nv, B, heads, Nq, Nk, d, qscale):
+    """The flash kernel on random q / k / v against an fp32 torch reference; qscale = 4 makes peaked rows (logit range
+    ~ +-30: exercises the flush of small exponentials and the lazy-rescale headroom), with d = 64 and a ragged last key
+    block."""
+    g = torch.Generator().manual_seed(100 + Nq)
     q = (qscale * torch.randn((B * heads, Nq, d), generator=g)).cuda().half()
     Nkp = (Nk + 7) // 8 * 8
     k = torch.zeros((B * heads, Nkp, d), device="cuda", dtype=torch.float16)
@@ -516,14 +472,7 @@ def test_flash_attention_polynomial_exp2(nv, pm, B, heads, Nq, Nk, d, qscale):
     vt[:, :, :Nk] = torch.randn((B * heads, d, Nk), generator=g).cuda().half()
     scale = d ** -0.5
     out0 = torch.empty((B, Nq, heads * d), device="cuda", dtype=torch.float16)
-    out1 = torch.empty_like(out0)
-    nv.set_env_option(None, None)
     nv.flash_attn(q, k, vt, B=B, heads=heads, Nq=Nq, Nk=Nk, scale=scale, out=out0)
-    try:
-        nv.set_env_option("flash_poly_mod", pm)
-        nv.flash_attn(q, k, vt, B=B, heads=heads, Nq=Nq, Nk=Nk, scale=scale, out=out1)
-    finally:
-        nv.set_env_option(None, None)
     torch.cuda.synchronize()
     s = torch.bmm(q.float(), k[:, :Nk].float().transpose(1, 2))
     if qscale == 1.0:
@@ -535,8 +484,3 @@ def test_flash_attention_polynomial_exp2(nv, pm, B, heads, Nq, Nk, d, qscale):
     ref = torch.bmm(torch.softmax(s, -1), vt[:, :, :Nk].float().transpose(1, 2))
     ref = ref.reshape(B, heads, Nq, d).permute(0, 2, 1, 3).reshape(B, Nq, heads * d)
     close(out0, ref, rtol=8e-3, atol=4e-3)
-    close(out1, ref, rtol=8e-3, atol=4e-3)
-    e0 = ((out0.float() - ref).pow(2).mean() / ref.pow(2).mean()).sqrt().item()
-    e1 = ((out1.float() - ref).pow(2).mean() / ref.pow(2).mean()).sqrt().item()
-    print(f"[flash poly] pm={pm} N={Nq}x{Nk} d={d}: rel rms MUFU {e0:.2e}  poly {e1:.2e}")
-    assert e1 < (3e-3 if pm == 1 else max(2.0 * e0, 1.5e-3))      # pm = 1: exponent argument rounded to fp16 (2^-8 abs near t = 8)

@@ -49,7 +49,7 @@ def main():
 
     # name -> callable applied before that variant's warm-up + capture (library switches, python-level toggles ...)
     variants = {"default": lambda: None}
-    for spec in args.env_variant:                      # e.g. --env-variant flash_poly=PFD_FLASH_POLY:1
+    for spec in args.env_variant:                      # e.g. --env-variant det=deterministic:1
         vname, kv = spec.split("=", 1)
         key, val = kv.split(":", 1)
         variants[vname] = (lambda k=key, v=val: nv.set_env_option(k, v))

@@ -1,4 +1,4 @@
-"""GroupNorm(+SiLU) device time on the UNet's shapes (graph-timed); default = two-pass kernels; PFD_GN_SOLO=1 / PFD_GN_CLUSTER=1 select the single-pass variants."""
+"""GroupNorm(+SiLU) device time on the UNet's batch-8 shapes (graph-timed), with a second, concatenated input where the UNet has a skip; the total weights each shape by how often the UNet runs it."""
 import json
 import os
 import sys
