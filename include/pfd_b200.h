@@ -401,6 +401,44 @@ PFD_API int pfd_pidinet_side_f32(const float* u, int32_t B, int32_t h, int32_t w
 PFD_API int pfd_pidinet_fuse_f32(const float* const* sides, const int32_t* side_h, const int32_t* side_w, int32_t B,
                                  int32_t H, int32_t W, const float* cls, float* out, void* stream);
 
+/*
+ * M-LSD, ControlNet.preprocess(type='mlsd' / 'mlsd_v11p') (controlnet.py:378-386 -> controlnet_annotator/mlsd:
+ * apply_mlsd, pred_lines and MobileV2_MLSD_Large).  Every conv of the network except the depthwise ones and the final
+ * 1x1 runs on pfd_gemm_f16 with BN folded into its weights.  All six are asynchronous on `stream` and graph-capturable
+ * (segment counts stay on the device), and each output depends on its own image only.
+ *
+ * pfd_mlsd_input_f16: NCHW [B,3,H,W] image in [0,1] (fp32 if x_f32, else fp16) -> channel-last fp16 [B,H,W,16] =
+ *   [u8 - 127.5 for r, g, b; 1 - 127.5 for the ones channel; 0 x 12] with u8 = x.mul(255).byte() (ToPILImage).  The
+ *   network's 1 / 127.5 belongs in the stem weights.
+ * pfd_mlsd_dw_f16: depthwise 3x3 ConvBNReLU6 (mbv2_mlsd_large.py:92-121): x [B,H,W,C] fp16 (C % 8 == 0), w fp32 [9][C]
+ *   (tap-major), b fp32 [C] -> out = clamp(conv(min(x, 6)) + b, 0, 6) fp16; stride 1: [B,H,W,C], padding 1; stride 2:
+ *   [B,H/2,W/2,C], F.pad(x, (0,1,0,1)) then padding 0.
+ * pfd_mlsd_upsample_f16: F.interpolate(scale_factor=2, bilinear, align_corners=True) of x [B,h,w,C] fp16 into out, an
+ *   [B,2h,2w] raster of fp16 pixels `pitch` elements apart (a channel slice of a wider tensor).
+ * pfd_mlsd_head_f32: x [B,h,w,C] fp16 (C % 8 == 0, C <= 256), w fp32 [5][C], b fp32 [5] -> out fp32 [B,5,h,w] =
+ *   w . x + b (the rows 7..11 of block23.conv3 that the decode reads).
+ * pfd_mlsd_decode_f32: deccode_output_score_and_ptss(maps, 200, 3) and the segment tests of pred_lines (utils.py:18-88):
+ *   maps fp32 [B,5,h,w] (centre logit, start x, y, end x, y displacements; h*w >= PFD_MLSD_TOPK) -> segs int32
+ *   [B,PFD_MLSD_TOPK,4] (x0, y0, x1, y1 image coordinates int(2 * (x + d)), float64, truncated) and count int32 [B].
+ *   A cell is a candidate when sigmoid(centre) is a 3x3 maximum and > thr_v; the top PFD_MLSD_TOPK candidates by score
+ *   (ties: lowest flat index) become segments when |start - end| > thr_d (float32), listed in flat-index order.  keys:
+ *   uint32 workspace [B*h*w].
+ * pfd_mlsd_draw_f32: cv2.line(img, p0, p1, 255, 1, LINE_8) of segs[n, 0..count[n]) on out, float32 [B,3,H,W], which
+ *   the caller zeroes: 1.0 on every pixel of OpenCV's clipLine + 8-connected LineIterator, on all three planes.
+ */
+#define PFD_MLSD_TOPK 200
+PFD_API int pfd_mlsd_input_f16(const void* x, int32_t x_f32, int32_t B, int32_t H, int32_t W, void* out, void* stream);
+PFD_API int pfd_mlsd_dw_f16(const void* x, int32_t B, int32_t H, int32_t W, int32_t C, int32_t stride, const float* w,
+                            const float* b, void* out, void* stream);
+PFD_API int pfd_mlsd_upsample_f16(const void* x, int32_t B, int32_t h, int32_t w, int32_t C, void* out, int64_t pitch,
+                                  void* stream);
+PFD_API int pfd_mlsd_head_f32(const void* x, int32_t B, int32_t h, int32_t w, int32_t C, const float* wt,
+                              const float* b, float* out, void* stream);
+PFD_API int pfd_mlsd_decode_f32(const float* maps, int32_t B, int32_t h, int32_t w, float thr_v, float thr_d,
+                                uint32_t* keys, int32_t* segs, int32_t* count, void* stream);
+PFD_API int pfd_mlsd_draw_f32(const int32_t* segs, const int32_t* count, int32_t B, int32_t H, int32_t W, float* out,
+                              void* stream);
+
 #ifdef __cplusplus
 }
 #endif

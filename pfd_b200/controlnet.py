@@ -5,9 +5,9 @@ Same constructor arguments / state-dict keys as the reference (spatial-transform
 ``UNetModel2D_Next.apply(control=...)``.  The hint stem (controlnet.py:165-181) depends only on the
 control image, so its output is cached per hint tensor instead of being recomputed every DDIM step.
 ``preprocess`` provides the annotator-free types on the GPU ('input', 'canny' — bit-exact cv2.Canny,
-SURVEY.md §8 f1), the HED soft-edge network ('hed', 'softedge_v11p', hed.py) and the scribble maps of methods 'pidinet'
-(the default, pidinet.py), 'hed' and 'xdog' (scribble.py); the other annotator networks (controlnet.py:361-503) are not
-implemented.
+SURVEY.md §8 f1), the HED soft-edge network ('hed', 'softedge_v11p', hed.py), the scribble maps of methods 'pidinet'
+(the default, pidinet.py), 'hed' and 'xdog' (scribble.py) and the M-LSD line maps ('mlsd', 'mlsd_v11p', mlsd.py); the
+other annotator networks (controlnet.py:361-503) are not implemented.
 """
 from __future__ import annotations
 
@@ -171,10 +171,12 @@ class ControlNet(nn.Module):
         batch at once; weights from pfd_b200.hed.load_hed / set_network, see hed.py) and 'scribble' with
         method='pidinet' (the default: the PiDiNet network, then make_scribble; weights from
         pfd_b200.pidinet.load_pidinet / set_network, see pidinet.py), method='hed' (HED, then make_scribble) or
-        method='xdog' (threshold=32), see scribble.py.  x: [B,3,H,W] tensor in [0,1] or an image path.  Returns float32
-        [B,3,H,W] on x's device; `size=` is ignored, as in the reference.  The other annotator networks (midas, mlsd,
-        openpose) raise NotImplementedError, and so does method='pidinet' while no PiDiNet weights are installed; an
-        unknown scribble method raises ValueError."""
+        method='xdog' (threshold=32), see scribble.py, and 'mlsd' / 'mlsd_v11p' (the M-LSD line network and its
+        decode, thr_v=0.1, thr_d=0.1; weights from pfd_b200.mlsd.load_mlsd / set_network, see mlsd.py).  x: [B,3,H,W]
+        tensor in [0,1] or an image path.  Returns float32 [B,3,H,W] on x's device; `size=` is ignored, as in the
+        reference.  The other annotator networks (midas, openpose) raise NotImplementedError, and so do
+        method='pidinet' and 'mlsd' while their weights are not installed; an unknown scribble method raises
+        ValueError."""
         if type == "none" or type is None:
             return None
         if isinstance(x, str):
@@ -203,8 +205,11 @@ class ControlNet(nn.Module):
         if type == "scribble":
             from .scribble import preprocess_scribble
             return preprocess_scribble(x, kwargs.pop("method", "pidinet"), kwargs.pop("threshold", 32))
+        if type in ("mlsd", "mlsd_v11p"):
+            from .mlsd import preprocess_mlsd
+            return preprocess_mlsd(x, kwargs.pop("thr_v", 0.1), kwargs.pop("thr_d", 0.1))
         raise NotImplementedError(f"controlnet annotator '{type}' is not implemented in pfd_b200 (the GPU serves "
-                                  "'input', 'canny', 'hed' and 'scribble'); feed a ready control map "
+                                  "'input', 'canny', 'hed', 'scribble' and 'mlsd'); feed a ready control map "
                                   "(do_preprocess=False)")
 
     def get_device(self):

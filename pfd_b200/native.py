@@ -34,11 +34,13 @@ EXPORTS = [
     "pfd_timestep_embedding_ft_f16", "pfd_ksampler_step_f32", "pfd_ksampler_begin_step", "pfd_randn_f16",
     "pfd_scribble_hed_f32", "pfd_scribble_blur_u8", "pfd_scribble_xdog_f32",
     "pfd_pidinet_dw_f16", "pfd_pidinet_reduce_f16", "pfd_pidinet_cdcm_f16", "pfd_pidinet_side_f32",
-    "pfd_pidinet_fuse_f32",
+    "pfd_pidinet_fuse_f32", "pfd_mlsd_input_f16", "pfd_mlsd_dw_f16", "pfd_mlsd_upsample_f16", "pfd_mlsd_head_f32",
+    "pfd_mlsd_decode_f32", "pfd_mlsd_draw_f32",
 ]
 PFD_KSAMPLER_NCOEF = 6
 PFD_HED_MAX_SIDES = 5
 PFD_PIDINET_SIDE_PARAMS = 161
+PFD_MLSD_TOPK = 200
 
 
 class GemmDesc(ctypes.Structure):
@@ -155,6 +157,15 @@ def load() -> ctypes.CDLL:
     lib.pfd_pidinet_side_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]
     lib.pfd_pidinet_fuse_f32.argtypes = [POINTER(c_void_p), POINTER(c_int32), POINTER(c_int32), c_int32, c_int32,
                                          c_int32, c_void_p, c_void_p, c_void_p]
+    lib.pfd_mlsd_input_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]
+    lib.pfd_mlsd_dw_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p,
+                                    c_void_p]
+    lib.pfd_mlsd_upsample_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_int64, c_void_p]
+    lib.pfd_mlsd_head_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p,
+                                      c_void_p]
+    lib.pfd_mlsd_decode_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_float, c_float, c_void_p, c_void_p,
+                                        c_void_p, c_void_p]
+    lib.pfd_mlsd_draw_f32.argtypes = [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p]
     for name in EXPORTS:
         if hasattr(lib, name) and name not in ("pfd_version", "pfd_last_error", "pfd_launch_count",
                                                "pfd_canny_workspace_bytes"):
@@ -791,6 +802,95 @@ def pidinet_fuse(sides: Sequence[torch.Tensor], cls: torch.Tensor, H: int, W: in
     ws = (c_int32 * 4)(*[s.shape[2] for s in sides])
     _check(load().pfd_pidinet_fuse_f32(ptrs, hs, ws, B, H, W, cls.data_ptr(), out.data_ptr(), stream_ptr()),
            "pfd_pidinet_fuse_f32")
+    return out
+
+
+def mlsd_input(x: torch.Tensor) -> torch.Tensor:
+    """NCHW [B,3,H,W] image in [0,1] (fp16/fp32) -> channel-last fp16 [B,H,W,16] = [u8 - 127.5 (rgb), 1 - 127.5, 0 x 12]
+    with u8 = x.mul(255).byte() (pfd_mlsd_input_f16)."""
+    if x.dim() != 4 or x.shape[1] != 3 or not x.is_cuda or x.dtype not in (torch.float16, torch.float32):
+        raise RuntimeError(f"mlsd_input: expected a CUDA fp16/fp32 [B,3,H,W] image, got {tuple(x.shape)} {x.dtype}")
+    x = x.contiguous()
+    B, _, H, W = x.shape
+    out = torch.empty((B, H, W, 16), device=x.device, dtype=torch.float16)
+    _check(load().pfd_mlsd_input_f16(x.data_ptr(), int(x.dtype == torch.float32), B, H, W, out.data_ptr(),
+                                     stream_ptr()), "pfd_mlsd_input_f16")
+    return out
+
+
+def mlsd_dw(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, stride: int) -> torch.Tensor:
+    """Depthwise 3x3 ConvBNReLU6 of channel-last x [B,H,W,C] fp16 (min(x, 6) on the input), w CUDA fp32 [9, C], b [C];
+    stride 2 pads like TFLite -> [B,H/s,W/s,C] fp16 (pfd_mlsd_dw_f16)."""
+    _chk16(x, "mlsd_dw x")
+    _chk32(w, "mlsd_dw w")
+    _chk32(b, "mlsd_dw b")
+    x = x.contiguous()
+    B, H, W, C = x.shape
+    if tuple(w.shape) != (9, C) or b.numel() != C:
+        raise RuntimeError(f"mlsd_dw: weights {tuple(w.shape)} / bias {tuple(b.shape)} do not fit C={C}")
+    out = torch.empty((B, H // stride, W // stride, C), device=x.device, dtype=torch.float16)
+    _check(load().pfd_mlsd_dw_f16(x.data_ptr(), B, H, W, C, int(stride), w.data_ptr(), b.data_ptr(), out.data_ptr(),
+                                  stream_ptr()), "pfd_mlsd_dw_f16")
+    return out
+
+
+def mlsd_upsample(x: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """Bilinear x2 (align_corners=True) of x [B,h,w,C] fp16 into out, a [B,2h,2w,C] view whose pixels are out.stride(2)
+    elements apart (e.g. a channel slice of a concat buffer) (pfd_mlsd_upsample_f16)."""
+    _chk16(x, "mlsd_upsample x")
+    _chk16(out, "mlsd_upsample out")
+    x = x.contiguous()
+    B, h, w, C = x.shape
+    p = out.stride(2)
+    if tuple(out.shape) != (B, 2 * h, 2 * w, C) or out.stride(3) != 1 or out.stride(1) != 2 * w * p \
+            or out.stride(0) != 2 * h * out.stride(1):
+        raise RuntimeError(f"mlsd_upsample: out {tuple(out.shape)} / strides {out.stride()} do not fit x {tuple(x.shape)}")
+    _check(load().pfd_mlsd_upsample_f16(x.data_ptr(), B, h, w, C, out.data_ptr(), p, stream_ptr()),
+           "pfd_mlsd_upsample_f16")
+    return out
+
+
+def mlsd_head(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
+    """x [B,h,w,C] fp16 -> fp32 [B,5,h,w] = w . x + b, w CUDA fp32 [5, C], b [5] (pfd_mlsd_head_f32)."""
+    _chk16(x, "mlsd_head x")
+    _chk32(w, "mlsd_head w")
+    _chk32(b, "mlsd_head b")
+    x = x.contiguous()
+    B, h, wd, C = x.shape
+    if tuple(w.shape) != (5, C) or b.numel() != 5:
+        raise RuntimeError(f"mlsd_head: weights {tuple(w.shape)} / bias {tuple(b.shape)} do not fit C={C}")
+    out = torch.empty((B, 5, h, wd), device=x.device, dtype=torch.float32)
+    _check(load().pfd_mlsd_head_f32(x.data_ptr(), B, h, wd, C, w.data_ptr(), b.data_ptr(), out.data_ptr(),
+                                    stream_ptr()), "pfd_mlsd_head_f32")
+    return out
+
+
+def mlsd_decode(maps: torch.Tensor, thr_v: float, thr_d: float) -> Tuple[torch.Tensor, torch.Tensor]:
+    """fp32 maps [B,5,h,w] (centre logit, start / end displacements) -> (int32 segments [B,200,4] (x0, y0, x1, y1),
+    int32 counts [B]) on the device (pfd_mlsd_decode_f32); rows past count[n] are unspecified."""
+    _chk32(maps, "mlsd_decode maps")
+    if maps.dim() != 4 or maps.shape[1] != 5:
+        raise RuntimeError(f"mlsd_decode: expected [B,5,h,w] maps, got {tuple(maps.shape)}")
+    B, _, h, w = maps.shape
+    keys = torch.empty((B, h, w), device=maps.device, dtype=torch.int32)
+    segs = torch.empty((B, PFD_MLSD_TOPK, 4), device=maps.device, dtype=torch.int32)
+    count = torch.empty((B,), device=maps.device, dtype=torch.int32)
+    _check(load().pfd_mlsd_decode_f32(maps.data_ptr(), B, h, w, float(thr_v), float(thr_d), keys.data_ptr(),
+                                      segs.data_ptr(), count.data_ptr(), stream_ptr()), "pfd_mlsd_decode_f32")
+    return segs, count
+
+
+def mlsd_draw(segs: torch.Tensor, count: torch.Tensor, H: int, W: int) -> torch.Tensor:
+    """float32 [B,3,H,W], 1.0 on the cv2.line(..., 1, LINE_8) pixels of segs[n, :count[n]] (int32 [B,200,4], device
+    counts) and 0 elsewhere (pfd_mlsd_draw_f32)."""
+    if segs.dtype != torch.int32 or count.dtype != torch.int32 or not segs.is_cuda or not count.is_cuda \
+            or segs.dim() != 3 or tuple(segs.shape[1:]) != (PFD_MLSD_TOPK, 4) or count.numel() != segs.shape[0]:
+        raise RuntimeError(f"mlsd_draw: expected CUDA int32 segments [B,{PFD_MLSD_TOPK},4] and counts [B]")
+    segs, count = segs.contiguous(), count.contiguous()
+    B = segs.shape[0]
+    out = torch.zeros((B, 3, H, W), device=segs.device, dtype=torch.float32)
+    _check(load().pfd_mlsd_draw_f32(segs.data_ptr(), count.data_ptr(), B, H, W, out.data_ptr(), stream_ptr()),
+           "pfd_mlsd_draw_f32")
     return out
 
 
