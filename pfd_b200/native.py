@@ -432,8 +432,22 @@ def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: flo
 
 def softmax_(s: torch.Tensor, scale: float, *, bias: Optional[torch.Tensor] = None, nheads: int = 1,
              mask: Optional[torch.Tensor] = None, nwin: int = 1) -> torch.Tensor:
-    """In-place row softmax over s [batch, rows, cols] (see pfd_softmax_f16)."""
+    """In-place row softmax over s [batch, rows, cols] (see pfd_softmax_f16).  Rows may be padded (stride(1) >= cols)
+    but the batches must be packed; bias is [nheads, rows, cols] (picked by b % nheads) and mask [nwin, rows, cols]
+    (picked by (b / nheads) % nwin), both contiguous."""
+    _chk16(s, "softmax_: s")
+    if s.dim() != 3:
+        raise ValueError(f"softmax_: s must be [batch, rows, cols], got {tuple(s.shape)}")
     batch, rows, cols = s.shape
+    if s.stride(2) != 1 or s.stride(1) < cols or s.stride(0) != rows * s.stride(1):
+        raise ValueError(f"softmax_: s {tuple(s.shape)} needs unit column stride, a row pitch >= cols and packed "
+                         f"batches, got strides {s.stride()}")
+    for t, n, name in ((bias, nheads, "bias"), (mask, nwin, "mask")):
+        if t is not None:
+            _chk16(t, f"softmax_: {name}")
+            if tuple(t.shape) != (max(n, 1), rows, cols) or not t.is_contiguous():
+                raise ValueError(f"softmax_: {name} must be a contiguous [{max(n, 1)}, {rows}, {cols}] tensor, "
+                                 f"got {tuple(t.shape)} with strides {t.stride()}")
     _check(load().pfd_softmax_f16(s.data_ptr(), batch, rows, cols, s.stride(1), scale, _p(bias), nheads,
                                   _p(mask), nwin, stream_ptr()), "pfd_softmax_f16")
     return s
@@ -932,11 +946,38 @@ def patchify(img: torch.Tensor, P: int, kpad: int) -> torch.Tensor:
     return out
 
 
+def _check_flash_shapes(what: str, q_rows: int, k_rows: int, k_d: int, vt_d: int, vt_cols: int, d: int, Nq: int,
+                        Nk: int) -> None:
+    # the kernel's tensor maps take Nq / Nk rows and d channels per head at the given strides: anything beyond a
+    # head's rows is the next head's data (or past the allocation for the last head)
+    if not (0 < Nq <= q_rows and 0 < Nk <= min(k_rows, vt_cols)):
+        raise ValueError(f"{what}: Nq={Nq}, Nk={Nk} exceed q rows {q_rows}, k rows {k_rows} or V^T columns {vt_cols}")
+    if k_d != d or vt_d != d:
+        raise ValueError(f"{what}: head dims differ: q {d}, k {k_d}, V^T rows {vt_d}")
+
+
+def _check_flash_out(what: str, out: torch.Tensor, B: int, heads: int, Nq: int, d: int) -> None:
+    # the epilogue stores __half2 pairs at out + b*stride(0) + q*stride(1) + h*d + c (c even)
+    _chk16(out, f"{what}: out")
+    if (out.dim() != 3 or out.shape[0] != B or out.shape[1] < Nq or out.shape[2] < heads * d
+            or out.stride(2) != 1 or out.stride(0) % 2 or out.stride(1) % 2 or out.data_ptr() % 4):
+        raise ValueError(f"{what}: out must be a [{B}, >={Nq}, >={heads * d}] view with unit column stride, even row "
+                         f"and batch strides and a 4-byte aligned base, got {tuple(out.shape)} with strides "
+                         f"{out.stride()} at offset {out.storage_offset()}")
+
+
 def flash_attn(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, *, B: int, heads: int, Nq: int, Nk: int,
                scale: float, out: torch.Tensor) -> torch.Tensor:
     """Fused attention (see pfd_flash_attn_f16): q [BH, Nqp, d], k [BH, Nkp, d], vt [BH, d, Nkp] ->
     out [B, Nq, heads*d]."""
+    for t, name in ((q, "q"), (k, "k"), (vt, "vt")):
+        _chk16(t, f"flash_attn: {name}")
+        if t.dim() != 3 or t.shape[0] != B * heads or not t.is_contiguous():
+            raise ValueError(f"flash_attn: {name} must be a contiguous [B*heads={B * heads}, rows, cols] tensor, "
+                             f"got {tuple(t.shape)} with strides {t.stride()}")
     d = q.shape[2]
+    _check_flash_shapes("flash_attn", q.shape[1], k.shape[1], k.shape[2], vt.shape[1], vt.shape[2], d, Nq, Nk)
+    _check_flash_out("flash_attn", out, B, heads, Nq, d)
     _check(load().pfd_flash_attn_f16(q.data_ptr(), k.data_ptr(), vt.data_ptr(), out.data_ptr(), B, heads, Nq, Nk,
                                      d, q.shape[1], k.shape[1], scale, vt.shape[2], out.stride(0), out.stride(1),
                                      0, stream_ptr()), "pfd_flash_attn_f16")
@@ -947,7 +988,14 @@ def flash_attn_strided(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, *, Nq
                        out: torch.Tensor) -> torch.Tensor:
     """pfd_flash_attn_strided_f16: q, k strided views [B, heads, N(p), d]; vt strided view [B, heads, d, Nk(p)]
     (rows contiguous); out [B, Nq, heads*d]."""
+    for t, name in ((q, "q"), (k, "k"), (vt, "vt")):
+        _chk16(t, f"flash_attn_strided: {name}")
+        if t.dim() != 4 or t.shape[:2] != q.shape[:2] or t.stride(3) != 1:
+            raise ValueError(f"flash_attn_strided: {name} must be a [{', '.join(map(str, q.shape[:2]))}, rows, cols] "
+                             f"view with unit column stride, got {tuple(t.shape)} with strides {t.stride()}")
     B, heads, _, d = q.shape
+    _check_flash_shapes("flash_attn_strided", q.shape[2], k.shape[2], k.shape[3], vt.shape[2], vt.shape[3], d, Nq, Nk)
+    _check_flash_out("flash_attn_strided", out, B, heads, Nq, d)
     st = lambda t: (c_int64 * 3)(t.stride(0), t.stride(1), t.stride(2))
     _check(load().pfd_flash_attn_strided_f16(q.data_ptr(), k.data_ptr(), vt.data_ptr(), out.data_ptr(), B, heads, Nq,
                                              Nk, d, st(q), st(k), st(vt), scale, out.stride(0), out.stride(1),

@@ -9,6 +9,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from attention_ref import flash_check
+
 pytestmark = pytest.mark.gpu
 
 
@@ -401,6 +403,9 @@ def test_flash_attention(nv, B, heads, Nq, Nk, d):
     close(o_unfused, ref, rtol=6e-3, atol=2e-3)
     # flash path: probabilities rounded to fp16 -> ~2^-11 relative error
     close(o_flash, ref, rtol=8e-3, atol=4e-3)
+    # and against exact float64 attention with the bound derived from the kernel's arithmetic
+    flash_check(o_flash.reshape(B, Nq, heads, d).permute(0, 2, 1, 3).reshape(B * heads, Nq, d), q[:, :Nq], k[:, :Nk],
+                vt[:, :, :Nk].transpose(1, 2), scale, f"model B={B} h={heads} {Nq}x{Nk} d={d}")
 
 
 @pytest.mark.parametrize("B,heads,Nq,Nk,d", [(8, 8, 4096, 148, 40), (2, 8, 1000, 148, 40), (3, 4, 64, 148, 40),
@@ -455,6 +460,9 @@ def test_flash_attention_fused_qk_swapped_vt(nv, B, heads, N, d):
     sc = (torch.matmul(qf, kf.transpose(-1, -2)).half().float() * scale).half().float()
     ref = torch.matmul(torch.softmax(sc, -1), vf).permute(0, 2, 1, 3).reshape(B, N, C)
     close(o, ref, rtol=8e-3, atol=4e-3)
+    flash_check(o.reshape(B, N, heads, d).permute(0, 2, 1, 3).reshape(B * heads, N, d),
+                qk[:, :heads, :N].reshape(B * heads, N, d), qk[:, heads:, :N].reshape(B * heads, N, d),
+                vt4.transpose(2, 3).reshape(B * heads, N, d), scale, f"fused q|k B={B} h={heads} N={N} d={d}")
 
 
 @pytest.mark.parametrize("B,heads,Nq,Nk,d,qscale", [(2, 8, 4096, 4096, 40, 1.0), (2, 8, 1024, 148, 40, 1.0),
