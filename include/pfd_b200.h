@@ -128,8 +128,9 @@ PFD_API int pfd_gemm_f16(const pfd_gemm_desc* d);
  * Replaces: diffusion_utils.py:175-191 (GroupNorm32, eps 1e-5) + nn.SiLU (openaimodel.py:201-203,
  *   224-229, 2732-2734), attention.py:83-84 (eps 1e-6), autokl_modules.py:33-39,
  *   seecoder.py:359,383.
- * ws: scratch of at least NB*groups*16 + NB*4 bytes (fp64 sum / sum-of-squares per (image, group), then one
- *     32-bit arrival counter per image for the single-pass kernel),
+ * ws: scratch of at least NB*groups*16 + NB*4 bytes (fp64 sum / sum-of-squares per (image, group) of x - K, where
+ *     the pivot K is the group's first channel at the image's first pixel, then one 32-bit arrival counter per image
+ *     for the single-pass kernel),
  *     16-byte aligned.  zero_ws != 0: the call zeroes it first (one extra memset node); zero_ws == 0: the
  *     caller guarantees it is already zero (e.g. one bulk memset of many slots per network evaluation).
  * Deterministic mode (pfd_set_option "deterministic"): each CTA's statistics are combined in a fixed order into one

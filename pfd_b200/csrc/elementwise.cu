@@ -54,8 +54,11 @@ __device__ __forceinline__ float rh(float v) { return __half2float(__float2half_
 // (vecs = C/8) so a thread always owns the same channel vector and strides over pixels ->
 // consecutive threads read consecutive 16-byte vectors of one pixel (fully coalesced), per-channel
 // partial sums / affine coefficients live in registers, and nothing is recomputed per element.
-//   pass 1 (gn_stats): per-(image, group) sum / sum of squares -> fp64 atomics (one per group per CTA)
+//   pass 1 (gn_stats): per-(image, group) sum / sum of squares of d = x - K_g -> fp64 atomics (one per group per CTA)
 //   pass 2 (gn_apply): y = x * a[c] + b[c] (a = rstd*gamma, b = beta - mean*a) [+ SiLU] -> fp16
+// K_g, the pivot, is the group's first channel at pixel 0 of the image.  Variance does not change under a shift, and
+// the one-pass E[d^2] - E[d]^2 loses only (E[d] / std)^2 of the fp32 partial sums' precision instead of (mean / std)^2:
+// activations with a large common offset (VAE decoder, real checkpoints) keep a full-precision rstd.
 constexpr int GN_MAX_GROUPS = 32;
 
 __device__ __forceinline__ uint4 gn_load(const __half* __restrict__ x1, int c1, const __half* __restrict__ x2,
@@ -64,7 +67,52 @@ __device__ __forceinline__ uint4 gn_load(const __half* __restrict__ x1, int c1, 
   return __ldg(reinterpret_cast<const uint4*>(x2 + pixn * c2 + (c - c1)));
 }
 
-__global__ void __launch_bounds__(320)
+// pivot K_g of the group holding channel c of image n (HW pixels per image)
+__device__ __forceinline__ float gn_pivot(const __half* __restrict__ x1, int c1, const __half* __restrict__ x2,
+                                          int c2, long long HW, int n, int cpg, int c) {
+  const int gc = c / cpg * cpg;
+  const long long pixn = (long long)n * HW;
+  return __half2float(gc < c1 ? __ldg(x1 + pixn * c1 + gc) : __ldg(x2 + pixn * c2 + (gc - c1)));
+}
+
+// pivots of the groups a thread's 8-channel vector at channel c touches (two loads when a group spans >= 8 channels)
+__device__ __forceinline__ void gn_pivots(const __half* __restrict__ x1, int c1, const __half* __restrict__ x2, int c2,
+                                          long long HW, int n, int cpg, int c, float (&kp)[8]) {
+  if (cpg >= 8) {
+    const int gb = (c / cpg + 1) * cpg;     // first channel of the next group
+    const float k0 = gn_pivot(x1, c1, x2, c2, HW, n, cpg, c);
+    const float k1 = gb < c + 8 ? gn_pivot(x1, c1, x2, c2, HW, n, cpg, gb) : k0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) kp[i] = c + i < gb ? k0 : k1;
+  } else {
+#pragma unroll
+    for (int i = 0; i < 8; ++i) kp[i] = gn_pivot(x1, c1, x2, c2, HW, n, cpg, c + i);
+  }
+}
+
+// fold a thread's 8 per-channel sums into (at most eight) group bins, then one shared atomic per bin
+__device__ __forceinline__ void gn_fold_bins(const float (&sm)[8], const float (&sq)[8], int c, int cpg, float* s_sum,
+                                             float* s_sq) {
+  int g_prev = c / cpg;
+  float as = 0.f, aq = 0.f;
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const int g = (c + i) / cpg;
+    if (g != g_prev) {
+      atomicAdd(&s_sum[g_prev], as);
+      atomicAdd(&s_sq[g_prev], aq);
+      as = aq = 0.f;
+      g_prev = g;
+    }
+    as += sm[i];
+    aq += sq[i];
+  }
+  atomicAdd(&s_sum[g_prev], as);
+  atomicAdd(&s_sq[g_prev], aq);
+}
+
+// at least 3 CTAs per SM: keeps this HBM-bound pass at 64 registers (the pivots and the wide-row branch add pressure)
+__global__ void __launch_bounds__(320, 3)
 gn_stats_kernel(const __half* __restrict__ x1, int c1, const __half* __restrict__ x2, int c2,
                 long long HW, int groups, long long pix_per_cta, double* __restrict__ ws) {
   pdl_enter();
@@ -86,9 +134,10 @@ gn_stats_kernel(const __half* __restrict__ x1, int c1, const __half* __restrict_
   if (lanes >= 1) {
     const int v = threadIdx.x % vecs;
     const int c = v * 8;
-    float sm[8], sq[8];
+    float sm[8], sq[8], kp[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) sm[i] = sq[i] = 0.f;
+    gn_pivots(x1, c1, x2, c2, HW, n, cpg, c, kp);
     long long pix = p0 + threadIdx.x / vecs;
     for (; pix + 3 * lanes < p1; pix += 4 * lanes) {
       uint4 u[4];
@@ -100,8 +149,9 @@ gn_stats_kernel(const __half* __restrict__ x1, int c1, const __half* __restrict_
         unpack8(u[k], f);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          sm[i] += f[i];
-          sq[i] += f[i] * f[i];
+          const float d = f[i] - kp[i];
+          sm[i] += d;
+          sq[i] += d * d;
         }
       }
     }
@@ -110,41 +160,32 @@ gn_stats_kernel(const __half* __restrict__ x1, int c1, const __half* __restrict_
       unpack8(gn_load(x1, c1, x2, c2, (long long)n * HW + pix, c), f);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
-        sm[i] += f[i];
-        sq[i] += f[i] * f[i];
+        const float d = f[i] - kp[i];
+        sm[i] += d;
+        sq[i] += d * d;
       }
     }
-    // fold the 8 channels into (at most two) group bins, then one shared atomic per bin
-    int g_prev = c / cpg;
-    float as = 0.f, aq = 0.f;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const int g = (c + i) / cpg;
-      if (g != g_prev) {
-        atomicAdd(&s_sum[g_prev], as);
-        atomicAdd(&s_sq[g_prev], aq);
-        as = aq = 0.f;
-        g_prev = g;
-      }
-      as += sm[i];
-      aq += sq[i];
-    }
-    atomicAdd(&s_sum[g_prev], as);
-    atomicAdd(&s_sq[g_prev], aq);
+    gn_fold_bins(sm, sq, c, cpg, s_sum, s_sq);
   } else {
-    // very wide rows (vecs > blockDim): a thread walks several vectors of each pixel
-    for (long long pix = p0; pix < p1; ++pix) {
-      for (int v = threadIdx.x; v < vecs; v += blockDim.x) {
-        const int c = v * 8;
+    // very wide rows (vecs > blockDim): a thread owns vectors v, v + blockDim, ... and walks the chunk for each, so
+    // its sums stay per-thread in registers as on the narrow path (not one shared fp32 sum of the whole chunk)
+    for (int v = threadIdx.x; v < vecs; v += blockDim.x) {
+      const int c = v * 8;
+      float sm[8], sq[8], kp[8];
+#pragma unroll
+      for (int i = 0; i < 8; ++i) sm[i] = sq[i] = 0.f;
+      gn_pivots(x1, c1, x2, c2, HW, n, cpg, c, kp);
+      for (long long pix = p0; pix < p1; ++pix) {
         float f[8];
         unpack8(gn_load(x1, c1, x2, c2, (long long)n * HW + pix, c), f);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          const int g = (c + i) / cpg;
-          atomicAdd(&s_sum[g], f[i]);
-          atomicAdd(&s_sq[g], f[i] * f[i]);
+          const float d = f[i] - kp[i];
+          sm[i] += d;
+          sq[i] += d * d;
         }
       }
+      gn_fold_bins(sm, sq, c, cpg, s_sum, s_sq);
     }
   }
   __syncthreads();
@@ -194,9 +235,10 @@ gn_stats_det_kernel(const __half* __restrict__ x1, int c1, const __half* __restr
     if (threadIdx.x < lanes * vecs) {
       const int v = threadIdx.x % vecs, lane = threadIdx.x / vecs;
       const int c = v * 8;
-      float sm[8], sq[8];
+      float sm[8], sq[8], kp[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) sm[i] = sq[i] = 0.f;
+      gn_pivots(x1, c1, x2, c2, HW, n, cpg, c, kp);
       long long pix = p0 + lane;
       for (; pix + 3 * lanes < p1; pix += 4 * lanes) {
         uint4 u[4];
@@ -208,8 +250,9 @@ gn_stats_det_kernel(const __half* __restrict__ x1, int c1, const __half* __restr
           unpack8(u[k], f);
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
-            sm[i] += f[i];
-            sq[i] += f[i] * f[i];
+            const float d = f[i] - kp[i];
+            sm[i] += d;
+            sq[i] += d * d;
           }
         }
       }
@@ -218,8 +261,9 @@ gn_stats_det_kernel(const __half* __restrict__ x1, int c1, const __half* __restr
         unpack8(gn_load(x1, c1, x2, c2, base + pix, c), f);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          sm[i] += f[i];
-          sq[i] += f[i] * f[i];
+          const float d = f[i] - kp[i];
+          sm[i] += d;
+          sq[i] += d * d;
         }
       }
 #pragma unroll
@@ -232,16 +276,18 @@ gn_stats_det_kernel(const __half* __restrict__ x1, int c1, const __half* __restr
     // very wide rows (vecs > blockDim): a thread owns vectors v, v + blockDim, ... and walks the chunk for each
     for (int v = threadIdx.x; v < vecs; v += blockDim.x) {
       const int c = v * 8;
-      float sm[8], sq[8];
+      float sm[8], sq[8], kp[8];
 #pragma unroll
       for (int i = 0; i < 8; ++i) sm[i] = sq[i] = 0.f;
+      gn_pivots(x1, c1, x2, c2, HW, n, cpg, c, kp);
       for (long long pix = p0; pix < p1; ++pix) {
         float f[8];
         unpack8(gn_load(x1, c1, x2, c2, base + pix, c), f);
 #pragma unroll
         for (int i = 0; i < 8; ++i) {
-          sm[i] += f[i];
-          sq[i] += f[i] * f[i];
+          const float d = f[i] - kp[i];
+          sm[i] += d;
+          sq[i] += d * d;
         }
       }
 #pragma unroll
@@ -323,13 +369,13 @@ gn_apply_kernel(const __half* __restrict__ x1, int c1, const __half* __restrict_
       for (int i = 0; i < 8; ++i) {
         const int g = (c + i) / cpg;
         if (g != gprev) {
-          // fp64 only for the cancellation-prone E[x^2] - mean^2 (3 DP ops, no DP division)
+          // ws holds the sums of d = x - K_g: mean = K_g + E[d], var = E[d^2] - E[d]^2 (fp64, no DP division)
           const double s_sum = ws[((long long)n * groups + g) * 2 + 0];
           const double s_sq = ws[((long long)n * groups + g) * 2 + 1];
           const double m = s_sum * inv_cnt;
           double var = s_sq * inv_cnt - m * m;
           if (var < 0) var = 0;
-          mean = (float)m;
+          mean = (float)((double)gn_pivot(x1, c1, x2, c2, HW, n, cpg, c + i) + m);
           rstd = rsqrtf((float)var + eps);
           gprev = g;
         }
