@@ -440,6 +440,61 @@ PFD_API int pfd_mlsd_decode_f32(const float* maps, int32_t B, int32_t h, int32_t
 PFD_API int pfd_mlsd_draw_f32(const int32_t* segs, const int32_t* count, int32_t B, int32_t H, int32_t W, float* out,
                               void* stream);
 
+/* OpenPose body annotator, ControlNet.preprocess(type='openpose' / 'openpose_v11p') (controlnet.py:396-406 ->
+ * controlnet_annotator/openpose: Body.__call__ and util.draw_bodypose).  The network's 3x3 / 1x1 convs run on
+ * pfd_gemm_f16, its 7x7 convs on pfd_im2col7x7_f16 + pfd_gemm_f16.  Resize tables (idx int32 [D, T], weights [D, T])
+ * are OpenCV's, built on the host (pfd_b200/openpose_tables.py).
+ * pfd_openpose_input_f16: NCHW [B,3,H,W] image in [0,1] -> channel-last fp16 [B,hp,wp,16]: x.mul(255).byte(), BGR,
+ *   cv2.resize to h x w (mode 0 copy, 1 integer block mean fy x fx, 2 uint8 LANCZOS4 with int weights (8 taps), 3
+ *   INTER_AREA with float weights), padded to hp x wp with 128, u8 / 256 - 0.5; channels 3..15 are zero.
+ * pfd_openpose_pool_f16: 2x2 / stride 2 max pool of x [B,H,W,C] fp16 (C % 8 == 0).
+ * pfd_im2col7x7_f16: x [B,H,W,C] fp16 (C % 8 == 0) -> out [B*H*W, 49*C], k = tap * C + c, zero padding 3.
+ * pfd_openpose_head_f32: out[n, out_off + k, y, x] (planar fp32, out_c channels) = act(b[k] + w[k] . x[n,y,x,:]),
+ *   k < N, w fp32 [N][C], act = ReLU when relu.
+ * pfd_openpose_resize_f32: cv2.resize of channels c0..c0+C of planar fp32 src [B,src_c,hs,ws] to out [B,C,H,W]
+ *   (mode 0 copy / crop, 1 block mean fy x fx, 2 separable float tables).
+ * pfd_openpose_peaks_f32: heatmaps fp32 [B,18,H,W] -> scipy gaussian_filter(sigma 3) in float64 (gauss: 13 weights,
+ *   centre first; tmp, blur: float64 [B,18,H,W]; rowcnt int32 [B*18*H]), then the peaks (>= their 4 neighbours, 0
+ *   outside, and > 0.1) in raster order: xy int32 [B,18,PFD_OPENPOSE_MAX_PEAKS,2] (x, y), score float64 (the
+ *   unblurred value) and total int32 [B,18], the number of peaks found.  Peaks past PFD_OPENPOSE_MAX_PEAKS in raster
+ *   order are dropped; total - PFD_OPENPOSE_MAX_PEAKS of them when total exceeds it.
+ * pfd_openpose_assemble_f32: PAF scoring, greedy limb matching and person assembly (body.py:127-229).  up: planar fp32
+ *   [B,57,hs,ws] (38 PAF channels, then 19 heatmap channels) at the resized-image size, brought to H x W pointwise by
+ *   (mode, fy, fx, tables) as in pfd_openpose_resize_f32; conn float64 [B,19,MAX_PEAKS^2] and rows float64
+ *   [B,MAX_PERSONS,20] are workspaces.  persons int32 [B,MAX_PERSONS,18] (per part the peak's index in its part, or
+ *   -1), pscore float64 [B,MAX_PERSONS,2] (total score, parts) and npersons int32 [B].  Where the reference would
+ *   raise IndexError (a connection matching a third person row), the first two matching rows are used.
+ * pfd_openpose_draw_f32: util.draw_bodypose of every person on a zero canvas: out float32 [B,3,H,W] = colour / 255
+ *   (colors uint8 [35,3]: 17 limb colours, then 18 keypoint colours; sintab: OpenCV's 451-entry sine table; idx
+ *   int32 [B,H,W] workspace).
+ */
+#define PFD_OPENPOSE_MAX_PEAKS 128
+#define PFD_OPENPOSE_MAX_PERSONS (17 * PFD_OPENPOSE_MAX_PEAKS)
+PFD_API int pfd_openpose_input_f16(const void* x, int32_t x_f32, int32_t B, int32_t H, int32_t W, int32_t h, int32_t w,
+                                   int32_t hp, int32_t wp, int32_t mode, int32_t fy, int32_t fx, const int32_t* iy,
+                                   const void* wy, int32_t ty, const int32_t* ix, const void* wx, int32_t tx, void* out,
+                                   void* stream);
+PFD_API int pfd_openpose_pool_f16(const void* x, int32_t B, int32_t H, int32_t W, int32_t C, void* out, void* stream);
+PFD_API int pfd_im2col7x7_f16(const void* x, int32_t B, int32_t H, int32_t W, int32_t C, void* out, void* stream);
+PFD_API int pfd_openpose_head_f32(const void* x, int32_t B, int32_t h, int32_t w, int32_t C, const float* wt,
+                                  const float* b, int32_t N, int32_t relu, float* out, int32_t out_c, int32_t out_off,
+                                  void* stream);
+PFD_API int pfd_openpose_resize_f32(const float* src, int32_t B, int32_t src_c, int32_t c0, int32_t C, int32_t hs,
+                                    int32_t ws, int32_t H, int32_t W, int32_t mode, int32_t fy, int32_t fx,
+                                    const int32_t* iy, const float* wy, int32_t ty, const int32_t* ix, const float* wx,
+                                    int32_t tx, float* out, void* stream);
+PFD_API int pfd_openpose_peaks_f32(const float* maps, int32_t B, int32_t H, int32_t W, const double* gauss, double* tmp,
+                                   double* blur, int32_t* rowcnt, int32_t* xy, double* score, int32_t* total,
+                                   void* stream);
+PFD_API int pfd_openpose_assemble_f32(const float* up, int32_t B, int32_t up_c, int32_t hs, int32_t ws, int32_t H,
+                                      int32_t W, int32_t mode, int32_t fy, int32_t fx, const int32_t* iy,
+                                      const float* wy, int32_t ty, const int32_t* ix, const float* wx, int32_t tx,
+                                      const int32_t* total, const int32_t* xy, const double* score, double* conn,
+                                      double* rows, int32_t* persons, double* pscore, int32_t* npersons, void* stream);
+PFD_API int pfd_openpose_draw_f32(const int32_t* persons, const int32_t* npersons, const int32_t* xy, int32_t B,
+                                  int32_t H, int32_t W, const float* sintab, const uint8_t* colors, int32_t* idx,
+                                  float* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -172,11 +172,12 @@ class ControlNet(nn.Module):
         method='pidinet' (the default: the PiDiNet network, then make_scribble; weights from
         pfd_b200.pidinet.load_pidinet / set_network, see pidinet.py), method='hed' (HED, then make_scribble) or
         method='xdog' (threshold=32), see scribble.py, and 'mlsd' / 'mlsd_v11p' (the M-LSD line network and its
-        decode, thr_v=0.1, thr_d=0.1; weights from pfd_b200.mlsd.load_mlsd / set_network, see mlsd.py).  x: [B,3,H,W]
-        tensor in [0,1] or an image path.  Returns float32 [B,3,H,W] on x's device; `size=` is ignored, as in the
-        reference.  The other annotator networks (midas, openpose) raise NotImplementedError, and so do
-        method='pidinet' and 'mlsd' while their weights are not installed; an unknown scribble method raises
-        ValueError."""
+        decode, thr_v=0.1, thr_d=0.1; weights from pfd_b200.mlsd.load_mlsd / set_network, see mlsd.py) and 'openpose' /
+        'openpose_v11p' (the OpenPose body network, its decode and drawing; weights from
+        pfd_b200.openpose.load_openpose / set_network, see openpose.py).  x: [B,3,H,W] tensor in [0,1] or an image path.
+        Returns float32 [B,3,H,W] on x's device; `size=` is ignored, as in the reference.  The other annotators (midas,
+        openpose with face / hand) raise NotImplementedError, and so do method='pidinet', 'mlsd' and 'openpose' while
+        their weights are not installed; an unknown scribble method raises ValueError."""
         if type == "none" or type is None:
             return None
         if isinstance(x, str):
@@ -208,9 +209,15 @@ class ControlNet(nn.Module):
         if type in ("mlsd", "mlsd_v11p"):
             from .mlsd import preprocess_mlsd
             return preprocess_mlsd(x, kwargs.pop("thr_v", 0.1), kwargs.pop("thr_d", 0.1))
+        if type in ("openpose", "openpose_v11p"):
+            from .openpose import preprocess_openpose
+            return preprocess_openpose(x)
+        if type is not None and type.startswith("openpose_with"):
+            raise NotImplementedError(f"controlnet annotator '{type}' needs the OpenPose hand / face networks, which "
+                                      "pfd_b200 does not implement; type='openpose' runs the body annotator on the GPU")
         raise NotImplementedError(f"controlnet annotator '{type}' is not implemented in pfd_b200 (the GPU serves "
-                                  "'input', 'canny', 'hed', 'scribble' and 'mlsd'); feed a ready control map "
-                                  "(do_preprocess=False)")
+                                  "'input', 'canny', 'hed', 'scribble', 'mlsd' and 'openpose'); feed a ready control "
+                                  "map (do_preprocess=False)")
 
     def get_device(self):
         return self.time_embed[0].weight.device

@@ -35,12 +35,16 @@ EXPORTS = [
     "pfd_scribble_hed_f32", "pfd_scribble_blur_u8", "pfd_scribble_xdog_f32",
     "pfd_pidinet_dw_f16", "pfd_pidinet_reduce_f16", "pfd_pidinet_cdcm_f16", "pfd_pidinet_side_f32",
     "pfd_pidinet_fuse_f32", "pfd_mlsd_input_f16", "pfd_mlsd_dw_f16", "pfd_mlsd_upsample_f16", "pfd_mlsd_head_f32",
-    "pfd_mlsd_decode_f32", "pfd_mlsd_draw_f32",
+    "pfd_mlsd_decode_f32", "pfd_mlsd_draw_f32", "pfd_openpose_input_f16", "pfd_openpose_pool_f16", "pfd_im2col7x7_f16",
+    "pfd_openpose_head_f32", "pfd_openpose_resize_f32", "pfd_openpose_peaks_f32", "pfd_openpose_assemble_f32",
+    "pfd_openpose_draw_f32",
 ]
 PFD_KSAMPLER_NCOEF = 6
 PFD_HED_MAX_SIDES = 5
 PFD_PIDINET_SIDE_PARAMS = 161
 PFD_MLSD_TOPK = 200
+PFD_OPENPOSE_MAX_PEAKS = 128
+PFD_OPENPOSE_MAX_PERSONS = 17 * PFD_OPENPOSE_MAX_PEAKS
 
 
 class GemmDesc(ctypes.Structure):
@@ -166,6 +170,18 @@ def load() -> ctypes.CDLL:
     lib.pfd_mlsd_decode_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_float, c_float, c_void_p, c_void_p,
                                         c_void_p, c_void_p]
     lib.pfd_mlsd_draw_f32.argtypes = [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p]
+    lib.pfd_openpose_input_f16.argtypes = [c_void_p] + [c_int32] * 11 + [c_void_p, c_void_p, c_int32] * 2 + \
+        [c_void_p, c_void_p]
+    lib.pfd_openpose_pool_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]
+    lib.pfd_im2col7x7_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]
+    lib.pfd_openpose_head_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_int32,
+                                          c_int32, c_void_p, c_int32, c_int32, c_void_p]
+    lib.pfd_openpose_resize_f32.argtypes = [c_void_p] + [c_int32] * 11 + [c_void_p, c_void_p, c_int32] * 2 + \
+        [c_void_p, c_void_p]
+    lib.pfd_openpose_peaks_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32] + [c_void_p] * 8
+    lib.pfd_openpose_assemble_f32.argtypes = [c_void_p] + [c_int32] * 9 + [c_void_p, c_void_p, c_int32] * 2 + \
+        [c_void_p] * 9
+    lib.pfd_openpose_draw_f32.argtypes = [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32] + [c_void_p] * 5
     for name in EXPORTS:
         if hasattr(lib, name) and name not in ("pfd_version", "pfd_last_error", "pfd_launch_count",
                                                "pfd_canny_workspace_bytes"):
@@ -905,6 +921,135 @@ def mlsd_draw(segs: torch.Tensor, count: torch.Tensor, H: int, W: int) -> torch.
     out = torch.zeros((B, 3, H, W), device=segs.device, dtype=torch.float32)
     _check(load().pfd_mlsd_draw_f32(segs.data_ptr(), count.data_ptr(), B, H, W, out.data_ptr(), stream_ptr()),
            "pfd_mlsd_draw_f32")
+    return out
+
+
+def openpose_input(x: torch.Tensor, h: int, w: int, hp: int, wp: int, plan, tabs) -> torch.Tensor:
+    """NCHW [B,3,H,W] image in [0,1] -> channel-last fp16 [B,hp,wp,16]: u8 = x.mul(255).byte(), BGR, cv2.resize to
+    h x w by ``plan`` (openpose_tables.resize_plan; ``tabs`` its device tables), 128 pad, u8 / 256 - 0.5
+    (pfd_openpose_input_f16)."""
+    if x.dim() != 4 or x.shape[1] != 3 or not x.is_cuda or x.dtype not in (torch.float16, torch.float32):
+        raise RuntimeError(f"openpose_input: expected a CUDA fp16/fp32 [B,3,H,W] image, got {tuple(x.shape)} {x.dtype}")
+    x = x.contiguous()
+    B, _, H, W = x.shape
+    out = torch.empty((B, hp, wp, 16), device=x.device, dtype=torch.float16)
+    mode, fy, fx, ay, ax = _plan_args(plan, tabs, u8=True)
+    _check(load().pfd_openpose_input_f16(x.data_ptr(), int(x.dtype == torch.float32), B, H, W, h, w, hp, wp, mode, fy,
+                                         fx, *ay, *ax, out.data_ptr(), stream_ptr()), "pfd_openpose_input_f16")
+    return out
+
+
+def _plan_args(plan, tabs, u8: bool = False):
+    """(mode, fy, fx, (iy, wy, ty), (ix, wx, tx)) of a resize plan for the openpose kernels."""
+    none = (None, None, 0)
+    if plan[0] == "copy":
+        return 0, 0, 0, none, none
+    if plan[0] == "block":
+        return 1, plan[1], plan[2], none, none
+    (iy, wy), (ix, wx) = tabs
+    mode = (2 if wy.dtype == torch.int32 else 3) if u8 else 2
+    return mode, 0, 0, (iy.data_ptr(), wy.data_ptr(), iy.shape[1]), (ix.data_ptr(), wx.data_ptr(), ix.shape[1])
+
+
+def openpose_pool(x: torch.Tensor) -> torch.Tensor:
+    """2x2 / stride 2 max pool of x [B,H,W,C] fp16 (pfd_openpose_pool_f16)."""
+    _chk16(x, "openpose_pool x")
+    x = x.contiguous()
+    B, H, W, C = x.shape
+    out = torch.empty((B, H // 2, W // 2, C), device=x.device, dtype=torch.float16)
+    _check(load().pfd_openpose_pool_f16(x.data_ptr(), B, H, W, C, out.data_ptr(), stream_ptr()), "pfd_openpose_pool_f16")
+    return out
+
+
+def im2col7x7(x: torch.Tensor) -> torch.Tensor:
+    """x [B,H,W,C] fp16 -> [B*H*W, 49*C] rows of the 7x7 / pad 3 neighbourhood, k = tap * C + c (pfd_im2col7x7_f16)."""
+    _chk16(x, "im2col7x7 x")
+    x = x.contiguous()
+    B, H, W, C = x.shape
+    out = torch.empty((B * H * W, 49 * C), device=x.device, dtype=torch.float16)
+    _check(load().pfd_im2col7x7_f16(x.data_ptr(), B, H, W, C, out.data_ptr(), stream_ptr()), "pfd_im2col7x7_f16")
+    return out
+
+
+def openpose_head(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, relu: bool, out: torch.Tensor, off: int) -> None:
+    """out[:, off:off+N] (planar fp32 [B,C_out,h,w]) = act(w . x + b) of x [B,h,w,C] fp16, w fp32 [N, C]
+    (pfd_openpose_head_f32)."""
+    _chk16(x, "openpose_head x")
+    _chk32(w, "openpose_head w")
+    _chk32(b, "openpose_head b")
+    _chk32(out, "openpose_head out")
+    x = x.contiguous()
+    B, h, wd, C = x.shape
+    N = w.shape[0]
+    if w.shape[1] != C or b.numel() != N or out.shape[0] != B or tuple(out.shape[2:]) != (h, wd):
+        raise RuntimeError(f"openpose_head: weights {tuple(w.shape)} / out {tuple(out.shape)} do not fit x {tuple(x.shape)}")
+    _check(load().pfd_openpose_head_f32(x.data_ptr(), B, h, wd, C, w.data_ptr(), b.data_ptr(), N, int(relu),
+                                        out.data_ptr(), out.shape[1], off, stream_ptr()), "pfd_openpose_head_f32")
+
+
+def openpose_resize(src: torch.Tensor, c0: int, C: int, H: int, W: int, plan, tabs) -> torch.Tensor:
+    """cv2.resize of channels c0..c0+C of planar fp32 src [B,Cs,hs,ws] to [B,C,H,W] (pfd_openpose_resize_f32); a
+    'copy' plan to a smaller H x W is the top-left crop."""
+    _chk32(src, "openpose_resize src")
+    B, Cs, hs, ws = src.shape
+    out = torch.empty((B, C, H, W), device=src.device, dtype=torch.float32)
+    mode, fy, fx, ay, ax = _plan_args(plan, tabs)
+    _check(load().pfd_openpose_resize_f32(src.data_ptr(), B, Cs, c0, C, hs, ws, H, W, mode, fy, fx, *ay, *ax,
+                                          out.data_ptr(), stream_ptr()), "pfd_openpose_resize_f32")
+    return out
+
+
+def openpose_peaks(maps: torch.Tensor, gauss: torch.Tensor):
+    """Heatmaps fp32 [B,18,H,W] -> (xy int32 [B,18,MAX_PEAKS,2], score float64 [B,18,MAX_PEAKS], total int32 [B,18])
+    after the float64 Gaussian (gauss: CUDA float64 [13]) (pfd_openpose_peaks_f32)."""
+    _chk32(maps, "openpose_peaks maps")
+    B, P, H, W = maps.shape
+    if P != 18 or gauss.dtype != torch.float64 or gauss.numel() != 13:
+        raise RuntimeError(f"openpose_peaks: expected [B,18,H,W] maps and 13 float64 weights, got {tuple(maps.shape)}")
+    dev = maps.device
+    tmp = torch.empty((B, 18, H, W), device=dev, dtype=torch.float64)
+    blur = torch.empty_like(tmp)
+    rowcnt = torch.empty((B * 18 * H,), device=dev, dtype=torch.int32)
+    xy = torch.zeros((B, 18, PFD_OPENPOSE_MAX_PEAKS, 2), device=dev, dtype=torch.int32)
+    score = torch.zeros((B, 18, PFD_OPENPOSE_MAX_PEAKS), device=dev, dtype=torch.float64)
+    total = torch.empty((B, 18), device=dev, dtype=torch.int32)
+    _check(load().pfd_openpose_peaks_f32(maps.data_ptr(), B, H, W, gauss.data_ptr(), tmp.data_ptr(), blur.data_ptr(),
+                                         rowcnt.data_ptr(), xy.data_ptr(), score.data_ptr(), total.data_ptr(),
+                                         stream_ptr()), "pfd_openpose_peaks_f32")
+    return xy, score, total
+
+
+def openpose_assemble(up: torch.Tensor, H: int, W: int, plan, tabs, total: torch.Tensor, xy: torch.Tensor,
+                      score: torch.Tensor):
+    """PAF scoring, limb matching and person assembly (pfd_openpose_assemble_f32) -> (persons int32 [B,MAX_PERSONS,18],
+    pscore float64 [B,MAX_PERSONS,2], npersons int32 [B]).  up: planar fp32 [B,57,hs,ws]."""
+    _chk32(up, "openpose_assemble up")
+    B, C, hs, ws = up.shape
+    dev = up.device
+    P, R = PFD_OPENPOSE_MAX_PEAKS, PFD_OPENPOSE_MAX_PERSONS
+    conn = torch.empty((B, 19, P * P), device=dev, dtype=torch.float64)
+    rows = torch.empty((B, R, 20), device=dev, dtype=torch.float64)
+    persons = torch.empty((B, R, 18), device=dev, dtype=torch.int32)
+    pscore = torch.empty((B, R, 2), device=dev, dtype=torch.float64)
+    npersons = torch.empty((B,), device=dev, dtype=torch.int32)
+    mode, fy, fx, ay, ax = _plan_args(plan, tabs)
+    _check(load().pfd_openpose_assemble_f32(up.data_ptr(), B, C, hs, ws, H, W, mode, fy, fx, *ay, *ax, total.data_ptr(),
+                                            xy.data_ptr(), score.data_ptr(), conn.data_ptr(), rows.data_ptr(),
+                                            persons.data_ptr(), pscore.data_ptr(), npersons.data_ptr(), stream_ptr()),
+           "pfd_openpose_assemble_f32")
+    return persons, pscore, npersons
+
+
+def openpose_draw(persons: torch.Tensor, npersons: torch.Tensor, xy: torch.Tensor, H: int, W: int,
+                  sintab: torch.Tensor, colors: torch.Tensor) -> torch.Tensor:
+    """util.draw_bodypose of every person -> float32 [B,3,H,W] canvas / 255 (pfd_openpose_draw_f32)."""
+    B = persons.shape[0]
+    dev = persons.device
+    idx = torch.empty((B, H, W), device=dev, dtype=torch.int32)
+    out = torch.empty((B, 3, H, W), device=dev, dtype=torch.float32)
+    _check(load().pfd_openpose_draw_f32(persons.data_ptr(), npersons.data_ptr(), xy.data_ptr(), B, H, W,
+                                        sintab.data_ptr(), colors.data_ptr(), idx.data_ptr(), out.data_ptr(),
+                                        stream_ptr()), "pfd_openpose_draw_f32")
     return out
 
 
