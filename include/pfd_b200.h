@@ -198,7 +198,7 @@ PFD_API int pfd_add_rowvec_f16(const void* a, const void* row, int64_t rows, int
  * device table coef[step*4 + {0..3}] = {a_t, a_prev, sigma_t, sqrt_one_minus_at} (fp32) indexed by
  * the device-side int *step so that a captured CUDA graph can be replayed for every step.
  * noise (optional, eta > 0, ddim.py:168-170): x_prev += sigma_t * noise * temperature with the reference's fp16
- * rounding order.  log_tab (optional): int32 slot per schedule index (-1 = none); the step's x_prev / pred_x0
+ * rounding order (guidance and temperature stay fp32, as python scalars do in torch).  log_tab (optional): int32 slot per schedule index (-1 = none); the step's x_prev / pred_x0
  * are also stored at log_xt / log_x0 + slot*half_n (the `intermediates` lists, ddim.py:122-124).
  */
 PFD_API int pfd_ddim_step_f16(const void* eps, const void* x, int64_t half_n, float guidance,
@@ -214,7 +214,7 @@ PFD_API int pfd_vae_posterior_f16(const void* moments, int32_t B, int32_t zc, in
                                   const float* noise, float scale, void* mean, void* logvar, void* stdv,
                                   void* sample, void* stream);
 
-/* Device-side loop header of one DDIM step (ddim.py:108-113): *step -= 1; t_out[0..nb) = ttab[*step].
+/* Device-side loop header of one DDIM step (ddim.py:108-113): *step = max(*step - 1, 0); t_out[0..nb) = ttab[*step].
  * Lets one CUDA graph hold several (or all) steps of the sampling loop with no host work in between. */
 PFD_API int pfd_ddim_begin_step(int32_t* step, const int64_t* ttab, int64_t* t_out, int32_t nb, void* stream);
 

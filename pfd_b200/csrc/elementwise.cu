@@ -678,18 +678,20 @@ __global__ void vae_posterior_kernel(const __half* __restrict__ mom, int B, int 
 // Start of one DDIM step inside a replayed CUDA graph: the device-side step counter walks the schedule backwards
 // (ddim.py:108-112: index = total - i - 1) and the timestep of that index is broadcast to the UNet's t input
 // (ddim.py:113 torch.full((bs,), step)), so a graph holding any number of steps needs no host work between steps.
+// The counter stops at 0, so a header run once too often leaves the next ddim_step on schedule index 0, not on -1.
 __global__ void ddim_begin_step_kernel(int* __restrict__ step, const long long* __restrict__ ttab,
                                        long long* __restrict__ t_out, int nb) {
   pdl_enter();
-  const int idx = *step - 1;
+  const int idx = max(*step - 1, 0);
   __syncthreads();
-  for (int i = threadIdx.x; i < nb; i += blockDim.x) t_out[i] = ttab[idx < 0 ? 0 : idx];
+  for (int i = threadIdx.x; i < nb; i += blockDim.x) t_out[i] = ttab[idx];
   if (threadIdx.x == 0) *step = idx;
 }
 
 // CFG combine + DDIM update with the reference's fp16 rounding sequence (ddim.py:150-171).
 // noise (optional, eta > 0): x_prev = a_prev.sqrt()*pred_x0 + dir_xt + sigma_t*noise*temperature, every product /
-// sum rounded to fp16 in the reference's evaluation order (ddim.py:166-170).
+// sum rounded to fp16 in the reference's evaluation order (ddim.py:166-170).  guidance and temperature are python
+// floats there: torch multiplies an fp16 tensor by a python scalar held in fp32, so neither is rounded to fp16.
 // log_tab (optional): slot per schedule index (-1 = not logged) of the `intermediates` lists (ddim.py:122-124);
 // the step's x_prev / pred_x0 are also written to log_xt / log_x0 [slot] so multi-step graphs need no host copy.
 __global__ void ddim_step_kernel(const __half* __restrict__ eps, const __half* __restrict__ x,
@@ -708,7 +710,7 @@ __global__ void ddim_step_kernel(const __half* __restrict__ eps, const __half* _
   const float sqrt_at = rh(sqrtf(a_t));
   const float sqrt_ap = rh(sqrtf(a_prev));
   const float dir_c = rh(sqrtf(rh(rh(1.f - a_prev) - rh(sigma * sigma))));
-  const float temp = rh(temperature);
+  const float temp = temperature;
   const int slot = log_tab ? log_tab[st] : -1;
   __half* lxt = slot >= 0 ? log_xt + (long long)slot * half_n : nullptr;
   __half* lx0 = slot >= 0 ? log_x0 + (long long)slot * half_n : nullptr;

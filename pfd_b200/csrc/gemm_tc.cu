@@ -111,6 +111,8 @@ __device__ __forceinline__ float fast_erf(float x) {
 // (max |error| 2.5e-5, tools/fit_gelu.py; fp16 resolution near 1 is 4.9e-4).  The polynomial is evaluated on
 // clamp(x, +-10) because c < 0 would flip its sign beyond |x| = 11.1; at |x| = 10 the sigmoid is already 0 / 1
 // to 3e-9.  9 FMA-pipe instructions + 2 MUFU per element against ~17 + 2 for the A&S erf form.
+// Outside [-8, 8] the error of x * sigmoid(...) against the exact GELU is below 3e-8 up to |x| = 10; beyond, the
+// clamped sigmoid is off by at most 3e-9, so the error is below 3e-9 |x| (1.9e-4 at x = -65504, where GELU is 0).
 __device__ __forceinline__ float gelu_sig(float x) {
   const float xc = fminf(fmaxf(x, -10.f), 10.f);
   const float x2 = xc * xc;
