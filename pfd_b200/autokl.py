@@ -258,11 +258,11 @@ class DiagonalGaussianDistribution(object):
 def cached_conv_in(conv: Conv2d, cz: int):
     """conv_in consumes the 8-channel (zero-padded) post_quant output: pack [O, 9*8] with zero columns
     for the pad channels so the im2col row (k = tap*8 + c) lines up."""
-    from .modules import _h, cached
+    from .modules import cached, fp16
 
     def build():
         o = conv.weight.shape[0]
         w = torch.zeros((o, 3, 3, 8), device=conv.weight.device, dtype=torch.float16)
-        w[..., :cz] = _h(conv.weight).permute(0, 2, 3, 1)
-        return w.reshape(o, 72).contiguous(), _h(conv.bias), 72
+        w[..., :cz] = fp16(conv.weight).permute(0, 2, 3, 1)
+        return w.reshape(o, 72).contiguous(), fp16(conv.bias), 72
     return cached(conv, "conv_in8", [conv.weight, conv.bias], build)

@@ -21,15 +21,10 @@
 
 namespace pfd {
 
-__device__ __forceinline__ void pdl_enter_c() {
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-}
-
 // to_u8<T> (common.h): ToPILImage's x.mul(255).byte()
 template <typename T>
 __global__ void canny_pack_kernel(const T* __restrict__ x, int B, int H, int W, uint32_t* __restrict__ rgbx) {
-  pdl_enter_c();
+  pdl_enter();
   const long long hw = (long long)H * W;
   const long long total = (long long)B * hw;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
@@ -43,14 +38,14 @@ __global__ void canny_pack_kernel(const T* __restrict__ x, int B, int H, int W, 
 // ToTensor(ToPILImage(x)): floor(x * 255) / 255 as float32 (controlnet.py:345-348, type 'input')
 template <typename T>
 __global__ void u8_roundtrip_kernel(const T* __restrict__ x, long long n, float* __restrict__ out) {
-  pdl_enter_c();
+  pdl_enter();
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     out[i] = (float)to_u8<T>(x[i]) / 255.f;
 }
 
 __global__ void canny_grad_kernel(const uint32_t* __restrict__ rgbx, int B, int H, int W,
                                   short2* __restrict__ dxy, unsigned short* __restrict__ mag) {
-  pdl_enter_c();
+  pdl_enter();
   const long long hw = (long long)H * W;
   const long long total = (long long)B * hw;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
@@ -86,7 +81,7 @@ __global__ void canny_grad_kernel(const uint32_t* __restrict__ rgbx, int B, int 
 
 __global__ void canny_nms_kernel(const short2* __restrict__ dxy, const unsigned short* __restrict__ mag, int B, int H,
                                  int W, int low, int high, unsigned char* __restrict__ map) {
-  pdl_enter_c();
+  pdl_enter();
   const long long hw = (long long)H * W;
   const long long total = (long long)B * hw;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
@@ -128,7 +123,7 @@ __global__ void canny_nms_kernel(const short2* __restrict__ dxy, const unsigned 
 constexpr int HT = 32;
 __global__ void __launch_bounds__(HT* HT)
 canny_hyst_kernel(unsigned char* __restrict__ map, int H, int W, int* __restrict__ changed) {
-  pdl_enter_c();
+  pdl_enter();
   __shared__ unsigned char t[HT + 2][HT + 2];
   unsigned char* img = map + (long long)blockIdx.z * H * W;
   const int x0 = blockIdx.x * HT, y0 = blockIdx.y * HT;
@@ -162,7 +157,7 @@ canny_hyst_kernel(unsigned char* __restrict__ map, int H, int W, int* __restrict
 }
 
 __global__ void canny_emit_kernel(const unsigned char* __restrict__ map, int B, int H, int W, float* __restrict__ out) {
-  pdl_enter_c();
+  pdl_enter();
   const long long hw = (long long)H * W;
   const long long total = (long long)B * hw;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
@@ -174,13 +169,6 @@ __global__ void canny_emit_kernel(const unsigned char* __restrict__ map, int B, 
     o[hw] = v;
     o[2 * hw] = v;
   }
-}
-
-static inline int grid1d(long long total) {
-  long long g = (total + 255) / 256;
-  const long long cap = (long long)num_sms() * 16;
-  if (g > cap) g = cap;
-  return (int)(g < 1 ? 1 : g);
 }
 
 static inline size_t align256(size_t v) { return (v + 255) & ~(size_t)255; }
@@ -211,7 +199,7 @@ extern "C" PFD_API int pfd_canny_f32(const void* x, int32_t src_is_f32, int32_t 
   unsigned short* mag = reinterpret_cast<unsigned short*>(ws + align256(px * 4) * 2);
   unsigned char* map = reinterpret_cast<unsigned char*>(ws + align256(px * 4) * 2 + align256(px * 2));
   int* flag = reinterpret_cast<int*>(ws + align256(px * 4) * 2 + align256(px * 2) + align256(px));
-  const int g = grid1d((long long)px);
+  const int g = grid_cap((long long)px, 256);
   if (src_is_f32)
     launch_k(canny_pack_kernel<float>, dim3(g), dim3(256), (size_t)0, st, static_cast<const float*>(x), (int)B, (int)H, (int)W, rgbx);
   else
@@ -248,8 +236,8 @@ extern "C" PFD_API int pfd_image_u8_roundtrip_f32(const void* x, int32_t src_is_
   if (!x || !out || n <= 0) return set_error("pfd_image_u8_roundtrip_f32: bad arguments");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (src_is_f32)
-    launch_k(u8_roundtrip_kernel<float>, dim3(grid1d(n)), dim3(256), (size_t)0, st, static_cast<const float*>(x), (long long)n, out);
+    launch_k(u8_roundtrip_kernel<float>, dim3(grid_cap(n, 256)), dim3(256), (size_t)0, st, static_cast<const float*>(x), (long long)n, out);
   else
-    launch_k(u8_roundtrip_kernel<__half>, dim3(grid1d(n)), dim3(256), (size_t)0, st, static_cast<const __half*>(x), (long long)n, out);
+    launch_k(u8_roundtrip_kernel<__half>, dim3(grid_cap(n, 256)), dim3(256), (size_t)0, st, static_cast<const __half*>(x), (long long)n, out);
   return check_launch("u8_roundtrip");
 }

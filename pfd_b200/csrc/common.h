@@ -1,4 +1,4 @@
-// Host-side shared helpers for the C-ABI translation units (error text, launch counter).
+// Shared helpers for the C-ABI translation units (error text, launch counter, launch geometry, kernel entry).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -28,8 +28,8 @@ inline int check_launch(const char* what) {
   return 0;
 }
 
-// Programmatic dependent launch: every pfd kernel begins with griddepcontrol.wait (see pdl_wait() in
-// ptx.cuh / elementwise.cu) so its CTAs may be scheduled while the previous kernel of the stream drains;
+// Programmatic dependent launch: every pfd kernel begins with griddepcontrol.wait (see pdl_enter() below
+// and pdl_wait() in ptx.cuh) so its CTAs may be scheduled while the previous kernel of the stream drains;
 // set PFD_NO_PDL=1 to launch with plain stream ordering.
 inline bool use_pdl() {
   static int v = -1;
@@ -57,6 +57,14 @@ inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, siz
 }
 
 #ifdef __CUDACC__
+// Programmatic dependent launch at a kernel's entry: block until the producer kernel has completed, then let the
+// consumer kernel start scheduling its CTAs (see launch_k).  The GEMM and attention kernels place the two halves
+// separately (pdl_wait / pdl_launch_dependents in ptx.cuh).
+__device__ __forceinline__ void pdl_enter() {
+  asm volatile("griddepcontrol.wait;" ::: "memory");
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+}
+
 // ToPILImage on a float tensor: pic.mul(255).byte() - the product is rounded in the tensor's dtype, then truncated
 // (torchvision ToPILImage, controlnet.py:339; shared by the Canny and HED annotators)
 template <typename T>
@@ -83,6 +91,16 @@ inline int num_sms() {
   }
   return n;
 }
+
+// Grid of a grid-stride kernel: ceil(work / per_block) blocks, at most 16 per SM, at least 1.
+inline int grid_cap(long long work, int per_block) {
+  long long g = (work + per_block - 1) / per_block;
+  const long long cap = (long long)num_sms() * 16;
+  if (g > cap) g = cap;
+  return (int)(g < 1 ? 1 : g);
+}
+
+inline bool misaligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
 
 // Deterministic mode (pfd_set_option "deterministic"; default from PFD_DETERMINISTIC=1 at load, see api.cu): every
 // summation order depends only on a sample's own shapes, never on the batch, the SM count or a race between CTAs.

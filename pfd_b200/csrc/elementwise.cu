@@ -14,13 +14,6 @@
 
 namespace pfd {
 
-__device__ __forceinline__ void pdl_enter() {
-  // programmatic dependent launch: block until the producer kernel has completed, then let the
-  // consumer kernel start scheduling its CTAs (see common.h: launch_k)
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-}
-
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -843,14 +836,6 @@ __global__ void patchify_kernel(const T* __restrict__ x, int B, int C, int H, in
   }
 }
 
-static inline int grid_for(long long total, int threads) {
-  long long g = (total + threads - 1) / threads;
-  const long long cap = (long long)num_sms() * 16;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return (int)g;
-}
-
 // Scratch of the deterministic GroupNorm statistics, one per device: GN_DET_MAX_NB arrival counters, then the fp64
 // partials [NB][groups][chunks].  Allocated (and the counters zeroed) by the first deterministic call on the device,
 // which must not be inside a stream capture - every graph-captured path of the package runs eagerly first.  The
@@ -1010,7 +995,7 @@ extern "C" PFD_API int pfd_upsample2x_f16(const void* x, int32_t NB, int32_t H, 
                                   void* stream) {
   if (C % 8) return set_error("pfd_upsample2x_f16: C=%d", C);
   const long long total = (long long)NB * 4 * H * W * (C / 8);
-  launch_k(upsample2x_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream), 
+  launch_k(upsample2x_kernel, dim3(grid_cap(total, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream), 
       static_cast<const uint4*>(x), NB, H, W, C / 8, static_cast<uint4*>(out));
   return check_launch("upsample2x");
 }
@@ -1020,16 +1005,16 @@ extern "C" PFD_API int pfd_nchw_to_nhwc_f16(const void* x, int32_t src_is_f32, i
   const long long total = (long long)NB * H * W * Cpad;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (src_is_f32)
-    launch_k(nchw_to_nhwc_kernel<float>, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), st, static_cast<const float*>(x), NB, C, H, W, Cpad, mul, add, static_cast<__half*>(out));
+    launch_k(nchw_to_nhwc_kernel<float>, dim3(grid_cap(total, 256)), dim3(256), (size_t)(0), st, static_cast<const float*>(x), NB, C, H, W, Cpad, mul, add, static_cast<__half*>(out));
   else
-    launch_k(nchw_to_nhwc_kernel<__half>, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), st, static_cast<const __half*>(x), NB, C, H, W, Cpad, mul, add, static_cast<__half*>(out));
+    launch_k(nchw_to_nhwc_kernel<__half>, dim3(grid_cap(total, 256)), dim3(256), (size_t)(0), st, static_cast<const __half*>(x), NB, C, H, W, Cpad, mul, add, static_cast<__half*>(out));
   return check_launch("nchw_to_nhwc");
 }
 
 extern "C" PFD_API int pfd_nhwc_to_nchw_f16(const void* x, int32_t NB, int32_t C, int32_t H, int32_t W, int32_t Cpad,
                                     float mul, float add, float lo, float hi, void* out, void* stream) {
   const long long total = (long long)NB * C * H * W;
-  launch_k(nhwc_to_nchw_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream), 
+  launch_k(nhwc_to_nchw_kernel, dim3(grid_cap(total, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream), 
       static_cast<const __half*>(x), NB, C, H, W, Cpad, mul, add, lo, hi, static_cast<__half*>(out));
   return check_launch("nhwc_to_nchw");
 }
@@ -1039,14 +1024,14 @@ extern "C" PFD_API int pfd_im2col3x3_f16(const void* x, int32_t NB, int32_t H, i
   if (Kpad < 9 * C || Kpad % 8) return set_error("pfd_im2col3x3_f16: Kpad=%d for C=%d", Kpad, C);
   const int Ho = (H + 2 - 3) / stride + 1, Wo = (W + 2 - 3) / stride + 1;
   const long long total = (long long)NB * Ho * Wo * Kpad;
-  launch_k(im2col3x3_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream), 
+  launch_k(im2col3x3_kernel, dim3(grid_cap(total, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream), 
       static_cast<const __half*>(x), NB, H, W, C, stride, Ho, Wo, Kpad, static_cast<__half*>(out));
   return check_launch("im2col3x3");
 }
 
 extern "C" PFD_API int pfd_axpby_f16(const void* a, float sa, const void* b, float sb, int64_t n, void* out,
                              void* stream) {
-  launch_k(axpby_kernel, dim3(grid_for(n, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream), 
+  launch_k(axpby_kernel, dim3(grid_cap(n, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream), 
       static_cast<const __half*>(a), sa, static_cast<const __half*>(b), sb, n, static_cast<__half*>(out));
   return check_launch("axpby");
 }
@@ -1054,7 +1039,7 @@ extern "C" PFD_API int pfd_axpby_f16(const void* a, float sa, const void* b, flo
 extern "C" PFD_API int pfd_add_rowvec_f16(const void* a, const void* row, int64_t rows, int32_t C, void* out,
                                   void* stream) {
   if (C % 8) return set_error("pfd_add_rowvec_f16: C=%d", C);
-  launch_k(add_rowvec_kernel, dim3(grid_for(rows * (C / 8), 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream), 
+  launch_k(add_rowvec_kernel, dim3(grid_cap(rows * (C / 8), 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream), 
       static_cast<const uint4*>(a), static_cast<const uint4*>(row), rows, C / 8, static_cast<uint4*>(out));
   return check_launch("add_rowvec");
 }
@@ -1065,7 +1050,7 @@ extern "C" PFD_API int pfd_ddim_step_f16(const void* eps, const void* x, int64_t
                                  void* log_x0, void* stream) {
   if (!eps || !x || !x_prev || !coef || half_n <= 0) return set_error("pfd_ddim_step_f16: null/empty argument");
   if (log_tab && (!log_xt || !log_x0)) return set_error("pfd_ddim_step_f16: log_tab without log buffers");
-  launch_k(ddim_step_kernel, dim3(grid_for(half_n, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream),
+  launch_k(ddim_step_kernel, dim3(grid_cap(half_n, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream),
       static_cast<const __half*>(eps), static_cast<const __half*>(x), half_n, guidance, coef, step,
       static_cast<__half*>(x_prev), static_cast<__half*>(pred_x0), static_cast<const __half*>(noise), temperature,
       log_tab, static_cast<__half*>(log_xt), static_cast<__half*>(log_x0));
@@ -1077,7 +1062,7 @@ extern "C" PFD_API int pfd_vae_posterior_f16(const void* moments, int32_t B, int
                                              void* logvar, void* stdv, void* sample, void* stream) {
   if (!moments || B <= 0 || zc <= 0 || cpad < 2 * zc) return set_error("pfd_vae_posterior_f16: bad arguments");
   const long long total = (long long)B * zc * H * W;
-  launch_k(vae_posterior_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream),
+  launch_k(vae_posterior_kernel, dim3(grid_cap(total, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream),
       static_cast<const __half*>(moments), (int)B, (int)zc, (int)H, (int)W, (int)cpad, noise, scale,
       static_cast<__half*>(mean), static_cast<__half*>(logvar), static_cast<__half*>(stdv), static_cast<__half*>(sample));
   return check_launch("vae_posterior");
@@ -1097,7 +1082,7 @@ extern "C" PFD_API int pfd_window_gather_f16(const void* x, int32_t B, int32_t H
   if (C % 8) return set_error("pfd_window_gather_f16: C=%d", C);
   const int Hp = (H + ws - 1) / ws * ws, Wp = (W + ws - 1) / ws * ws;
   const long long total = (long long)B * Hp * Wp * (C / 8);
-  launch_k(window_gather_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream), 
+  launch_k(window_gather_kernel, dim3(grid_cap(total, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream), 
       static_cast<const uint4*>(x), B, H, W, C / 8, ws, shift, Hp, Wp, static_cast<uint4*>(out));
   return check_launch("window_gather");
 }
@@ -1108,7 +1093,7 @@ extern "C" PFD_API int pfd_window_scatter_f16(const void* win, int32_t B, int32_
   if (C % 8) return set_error("pfd_window_scatter_f16: C=%d", C);
   const int Hp = (H + ws - 1) / ws * ws, Wp = (W + ws - 1) / ws * ws;
   const long long total = (long long)B * H * W * (C / 8);
-  launch_k(window_scatter_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream), 
+  launch_k(window_scatter_kernel, dim3(grid_cap(total, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream), 
       static_cast<const uint4*>(win), B, H, W, C / 8, ws, shift, Hp, Wp,
       static_cast<const uint4*>(residual), static_cast<uint4*>(out));
   return check_launch("window_scatter");
@@ -1118,7 +1103,7 @@ extern "C" PFD_API int pfd_patch_merge_gather_f16(const void* x, int32_t B, int3
                                           void* out, void* stream) {
   if (C % 8) return set_error("pfd_patch_merge_gather_f16: C=%d", C);
   const long long total = (long long)B * ((H + 1) / 2) * ((W + 1) / 2) * 4 * (C / 8);
-  launch_k(patch_merge_kernel, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream), 
+  launch_k(patch_merge_kernel, dim3(grid_cap(total, 256)), dim3(256), (size_t)(0), static_cast<cudaStream_t>(stream), 
       static_cast<const uint4*>(x), B, H, W, C / 8, static_cast<uint4*>(out));
   return check_launch("patch_merge");
 }
@@ -1129,8 +1114,8 @@ extern "C" PFD_API int pfd_patchify_f16(const void* x, int32_t src_is_f32, int32
   const long long total = (long long)B * ((H + P - 1) / P) * ((W + P - 1) / P) * Kpad;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (src_is_f32)
-    launch_k(patchify_kernel<float>, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), st, static_cast<const float*>(x), B, C, H, W, P, Kpad, static_cast<__half*>(out));
+    launch_k(patchify_kernel<float>, dim3(grid_cap(total, 256)), dim3(256), (size_t)(0), st, static_cast<const float*>(x), B, C, H, W, P, Kpad, static_cast<__half*>(out));
   else
-    launch_k(patchify_kernel<__half>, dim3(grid_for(total, 256)), dim3(256), (size_t)(0), st, static_cast<const __half*>(x), B, C, H, W, P, Kpad, static_cast<__half*>(out));
+    launch_k(patchify_kernel<__half>, dim3(grid_cap(total, 256)), dim3(256), (size_t)(0), st, static_cast<const __half*>(x), B, C, H, W, P, Kpad, static_cast<__half*>(out));
   return check_launch("patchify");
 }

@@ -22,23 +22,11 @@
 
 namespace pfd {
 
-__device__ __forceinline__ void pdl_enter_h() {
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-}
-
-static inline int grid_cap(long long work, int per_block) {
-  long long g = (work + per_block - 1) / per_block;
-  const long long cap = (long long)num_sms() * 16;
-  if (g > cap) g = cap;
-  return (int)(g < 1 ? 1 : g);
-}
-
 // out[n, y, x, c] = (u8(x[n, c, y, x]) - norm[c]) * scale for c < 3, 0 for the pad channels
 template <typename T>
 __global__ void hed_input_kernel(const T* __restrict__ x, int B, int H, int W, int Cpad, const float* __restrict__ norm,
                                  float scale, __half* __restrict__ out) {
-  pdl_enter_h();
+  pdl_enter();
   const float n0 = norm[0], n1 = norm[1], n2 = norm[2];
   const long long hw = (long long)H * W;
   const long long total = (long long)B * hw;
@@ -63,7 +51,7 @@ __global__ void __launch_bounds__(256)
 hed_pool_side_kernel(const __half* __restrict__ x, int B, int h, int w, int C, int L, const float* __restrict__ proj_w,
                      const float* __restrict__ proj_b, float* __restrict__ side, __half* __restrict__ pooled) {
   extern __shared__ float s_w[];
-  pdl_enter_h();
+  pdl_enter();
   for (int c = threadIdx.x; c < C; c += blockDim.x) s_w[c] = proj_w[c];
   __syncthreads();
   const float bias = *proj_b;
@@ -173,7 +161,7 @@ __device__ __forceinline__ float resize_linear(const float* __restrict__ s, int 
 }
 
 __global__ void hed_fuse_kernel(HedSides sd, int B, int H, int W, float inv_scale, float* __restrict__ out) {
-  pdl_enter_h();
+  pdl_enter();
   const long long hw = (long long)H * W;
   const long long total = (long long)B * hw;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
@@ -222,7 +210,7 @@ extern "C" PFD_API int pfd_hed_pool_side_f16(const void* x, int32_t B, int32_t h
                                              void* stream) {
   if (!x || !proj_w || !proj_b || !side || B <= 0 || h <= 0 || w <= 0 || C <= 0 || C % 8 || C > 8192)
     return set_error("pfd_hed_pool_side_f16: bad arguments (B=%d h=%d w=%d C=%d)", B, h, w, C);
-  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(pooled)) & 15)
+  if (misaligned(x) || misaligned(pooled))
     return set_error("pfd_hed_pool_side_f16: x and pooled must be 16-byte aligned");
   int L = 1;
   while (L < C / 8 && L < 32) L <<= 1;

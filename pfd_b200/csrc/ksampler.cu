@@ -12,15 +12,10 @@
 
 namespace pfd {
 
-__device__ __forceinline__ void pdl_enter_k() {
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-}
-
 // *step += 1; t_out[0..nb) = ttab[*step]  (the index is clamped to the table)
 __global__ void ksampler_begin_step_kernel(int* __restrict__ step, const float* __restrict__ ttab, int nsteps,
                                            float* __restrict__ t_out, int nb) {
-  pdl_enter_k();
+  pdl_enter();
   int idx = *step + 1;
   idx = idx < 0 ? 0 : (idx >= nsteps ? nsteps - 1 : idx);
   __syncthreads();
@@ -34,7 +29,7 @@ __global__ void ksampler_step_kernel(const __half* __restrict__ eps, int cfg, fl
                                      const __half* __restrict__ noise, __half* __restrict__ unet_in,
                                      __half* __restrict__ out, const int* __restrict__ log_tab,
                                      __half* __restrict__ log_xt, __half* __restrict__ log_x0) {
-  pdl_enter_k();
+  pdl_enter();
   const int st = *step;
   const float* row = coef + (long long)st * PFD_KSAMPLER_NCOEF;
   const float sigma = row[0], a = row[1], b = row[2], c = row[3], u = row[4], cin_next = row[5];
@@ -69,14 +64,6 @@ __global__ void ksampler_step_kernel(const __half* __restrict__ eps, int cfg, fl
   }
 }
 
-static inline int ks_grid(long long n) {
-  long long g = (n + 255) / 256;
-  const long long cap = (long long)num_sms() * 16;
-  if (g > cap) g = cap;
-  if (g < 1) g = 1;
-  return (int)g;
-}
-
 }  // namespace pfd
 
 using namespace pfd;
@@ -97,7 +84,7 @@ extern "C" PFD_API int pfd_ksampler_step_f32(const void* eps, int32_t cfg, float
   if (!eps || !coef || !step || !x || !d_prev || !unet_in || !out || half_n <= 0)
     return set_error("pfd_ksampler_step_f32: null/empty argument");
   if (log_tab && (!log_xt || !log_x0)) return set_error("pfd_ksampler_step_f32: log_tab without log buffers");
-  launch_k(ksampler_step_kernel, dim3(ks_grid(half_n)), dim3(256), (size_t)0, static_cast<cudaStream_t>(stream),
+  launch_k(ksampler_step_kernel, dim3(grid_cap(half_n, 256)), dim3(256), (size_t)0, static_cast<cudaStream_t>(stream),
            static_cast<const __half*>(eps), (int)(cfg != 0), guidance, (long long)half_n, coef,
            reinterpret_cast<const int*>(step), (int)last_step, x, d_prev, static_cast<const __half*>(noise),
            static_cast<__half*>(unet_in), static_cast<__half*>(out), reinterpret_cast<const int*>(log_tab),

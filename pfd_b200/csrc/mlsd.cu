@@ -28,6 +28,7 @@
 
 #include "../../include/pfd_b200.h"
 #include "common.h"
+#include "cvdraw.cuh"
 
 namespace pfd {
 
@@ -35,23 +36,11 @@ constexpr int MLSD_TOPK = PFD_MLSD_TOPK;
 constexpr int MLSD_CIN = 16;         // stem input channels: rgb, ones, 12 zero pads (the GEMM's 3x3 path needs >= 16)
 constexpr int SEL_THREADS = 1024;
 
-__device__ __forceinline__ void pdl_enter_m() {
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-}
-
-static inline int grid_cap_m(long long work, int per_block) {
-  long long g = (work + per_block - 1) / per_block;
-  const long long cap = (long long)num_sms() * 16;
-  if (g > cap) g = cap;
-  return (int)(g < 1 ? 1 : g);
-}
-
 // out[n, y, x, :] = [u8(r) - 127.5, u8(g) - 127.5, u8(b) - 127.5, 1 - 127.5, 0 x 12]
 template <typename T>
 __global__ void __launch_bounds__(256)
 mlsd_input_kernel(const T* __restrict__ x, int B, int H, int W, __half* __restrict__ out) {
-  pdl_enter_m();
+  pdl_enter();
   const long long hw = (long long)H * W, total = (long long)B * hw;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long n = i / hw, p = i % hw;
@@ -76,7 +65,7 @@ template <int S>
 __global__ void __launch_bounds__(256)
 mlsd_dw_kernel(const __half* __restrict__ x, int B, int H, int W, int C, const float* __restrict__ wt,
                const float* __restrict__ bias, __half* __restrict__ out) {
-  pdl_enter_m();
+  pdl_enter();
   const int Ho = S == 1 ? H : H / 2, Wo = S == 1 ? W : W / 2;
   const int V = C / 8;
   const long long total = (long long)B * Ho * Wo * V;
@@ -115,7 +104,7 @@ mlsd_dw_kernel(const __half* __restrict__ x, int B, int H, int W, int C, const f
 // with align_corners=True (scale = (in - 1) / (out - 1) in float32, source = scale * dst, second index clamped).
 __global__ void __launch_bounds__(256)
 mlsd_upsample_kernel(const __half* __restrict__ x, int B, int h, int w, int C, __half* __restrict__ out, long long pitch) {
-  pdl_enter_m();
+  pdl_enter();
   const int Ho = 2 * h, Wo = 2 * w, V = C / 8;
   const float sy = Ho > 1 ? (float)(h - 1) / (float)(Ho - 1) : 0.f;
   const float sx = Wo > 1 ? (float)(w - 1) / (float)(Wo - 1) : 0.f;
@@ -154,7 +143,7 @@ __global__ void __launch_bounds__(128)
 mlsd_head_kernel(const __half* __restrict__ x, int B, int h, int w, int C, const float* __restrict__ wt,
                  const float* __restrict__ bias, float* __restrict__ out) {
   extern __shared__ float s_w[];
-  pdl_enter_m();
+  pdl_enter();
   for (int i = threadIdx.x; i < 5 * C; i += blockDim.x) s_w[i] = wt[i];
   __syncthreads();
   const long long hw = (long long)h * w, total = (long long)B * hw;
@@ -185,7 +174,7 @@ __device__ __forceinline__ float mlsd_sigmoid(float v) { return __fdiv_rn(1.f, _
 // wins) and heat > thr_v, else 0.  Positive floats order like their bit patterns, so keys order like scores.
 __global__ void __launch_bounds__(256)
 mlsd_nms_kernel(const float* __restrict__ maps, int B, int h, int w, float thr_v, uint32_t* __restrict__ keys) {
-  pdl_enter_m();
+  pdl_enter();
   const long long hw = (long long)h * w, total = (long long)B * hw;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long n = i / hw, p = i % hw;
@@ -241,7 +230,7 @@ mlsd_select_kernel(const uint32_t* __restrict__ keys, const float* __restrict__ 
   __shared__ int s_scan[32];
   __shared__ uint32_t s_prefix, s_mask;
   __shared__ int s_rem, s_all;
-  pdl_enter_m();
+  pdl_enter();
   const int n = blockIdx.x;
   const long long hw = (long long)h * w;
   const uint32_t* K = keys + n * hw;
@@ -323,85 +312,28 @@ mlsd_select_kernel(const uint32_t* __restrict__ keys, const float* __restrict__ 
   if (threadIdx.x == 0) count[n] = out_base < MLSD_TOPK ? out_base : MLSD_TOPK;
 }
 
-// OpenCV's clipLine(Size(W, H), pt1, pt2) in int64 (drawing.cpp): false when the segment misses the image.
-__device__ bool mlsd_clip(long long W, long long H, long long& x1, long long& y1, long long& x2, long long& y2) {
-  const long long right = W - 1, bottom = H - 1;
-  int c1 = (x1 < 0) + (x1 > right) * 2 + (y1 < 0) * 4 + (y1 > bottom) * 8;
-  int c2 = (x2 < 0) + (x2 > right) * 2 + (y2 < 0) * 4 + (y2 > bottom) * 8;
-  if ((c1 & c2) == 0 && (c1 | c2) != 0) {
-    long long a;
-    if (c1 & 12) {
-      a = c1 < 8 ? 0 : bottom;
-      x1 += (long long)__ddiv_rn(__dmul_rn((double)(a - y1), (double)(x2 - x1)), (double)(y2 - y1));
-      y1 = a;
-      c1 = (x1 < 0) + (x1 > right) * 2;
-    }
-    if (c2 & 12) {
-      a = c2 < 8 ? 0 : bottom;
-      x2 += (long long)__ddiv_rn(__dmul_rn((double)(a - y2), (double)(x2 - x1)), (double)(y2 - y1));
-      y2 = a;
-      c2 = (x2 < 0) + (x2 > right) * 2;
-    }
-    if ((c1 & c2) == 0 && (c1 | c2) != 0) {
-      if (c1) {
-        a = c1 == 1 ? 0 : right;
-        y1 += (long long)__ddiv_rn(__dmul_rn((double)(a - x1), (double)(y2 - y1)), (double)(x2 - x1));
-        x1 = a;
-        c1 = 0;
-      }
-      if (c2) {
-        a = c2 == 1 ? 0 : right;
-        y2 += (long long)__ddiv_rn(__dmul_rn((double)(a - x2), (double)(y2 - y1)), (double)(x2 - x1));
-        x2 = a;
-        c2 = 0;
-      }
-    }
-  }
-  return (c1 | c2) == 0;
-}
-
-// One warp per segment slot (blockIdx.y = image).  After clipping and the left-to-right swap, LineIterator's pixel i
-// (i = 0..D along the major axis, D >= d the axis lengths) has taken m_i = ceil((2 d i - D) / 2D) minor steps: its
-// error term e_i = D - 2d(i + 1) + 2D m_i stays in [-2d, 2D - 2d), which fixes m_i.  out: [B,3,H,W], 1.0 on the line.
+// One warp per segment slot (blockIdx.y = image).  out: [B,3,H,W], 1.0 on the line.
 __global__ void __launch_bounds__(256)
 mlsd_draw_kernel(const int* __restrict__ segs, const int* __restrict__ count, int H, int W, float* __restrict__ out) {
-  pdl_enter_m();
+  pdl_enter();
   const int n = blockIdx.y;
   const int s = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32, lane = threadIdx.x & 31;
   if (s >= count[n]) return;
   const int* sg = segs + ((long long)n * MLSD_TOPK + s) * 4;
-  long long x1 = sg[0], y1 = sg[1], x2 = sg[2], y2 = sg[3];
-  if ((unsigned long long)x1 >= (unsigned long long)W || (unsigned long long)x2 >= (unsigned long long)W ||
-      (unsigned long long)y1 >= (unsigned long long)H || (unsigned long long)y2 >= (unsigned long long)H) {
-    if (!mlsd_clip(W, H, x1, y1, x2, y2)) return;
-  }
-  if (x2 < x1) {
-    long long t = x1; x1 = x2; x2 = t;
-    t = y1; y1 = y2; y2 = t;
-  }
-  const long long dx = x2 - x1, ady = y2 >= y1 ? y2 - y1 : y1 - y2;
-  const long long sy = y2 >= y1 ? 1 : -1;
-  const bool vert = ady > dx;
-  const long long D = vert ? ady : dx, d = vert ? dx : ady;
   const long long hw = (long long)H * W;
   float* o = out + (long long)n * 3 * hw;
-  for (long long i = lane; i <= D; i += 32) {
-    const long long a = 2 * d * i - D;
-    const long long m = D == 0 ? 0 : (a >= 0 ? (a + 2 * D - 1) / (2 * D) : -((-a) / (2 * D)));
-    const long long x = vert ? x1 + m : x1 + i, y = vert ? y1 + sy * i : y1 + sy * m;
-    if (x < 0 || x >= W || y < 0 || y >= H) continue;
+  for_each_line_pixel(W, H, sg[0], sg[1], sg[2], sg[3], lane, [&](long long x, long long y) {
     const long long p = y * W + x;
     o[p] = 1.f;
     o[hw + p] = 1.f;
     o[2 * hw + p] = 1.f;
-  }
+  });
 }
 
 }  // namespace pfd
 
 using namespace pfd;
 
-static bool misaligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
 
 extern "C" PFD_API int pfd_mlsd_input_f16(const void* x, int32_t x_f32, int32_t B, int32_t H, int32_t W, void* out,
                                           void* stream) {
@@ -409,7 +341,7 @@ extern "C" PFD_API int pfd_mlsd_input_f16(const void* x, int32_t x_f32, int32_t 
     return set_error("pfd_mlsd_input_f16: bad arguments (B=%d H=%d W=%d)", B, H, W);
   if (misaligned(out)) return set_error("pfd_mlsd_input_f16: out must be 16-byte aligned");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int g = grid_cap_m((long long)B * H * W, 256);
+  const int g = grid_cap((long long)B * H * W, 256);
   if (x_f32)
     launch_k(mlsd_input_kernel<float>, dim3(g), dim3(256), (size_t)0, st, static_cast<const float*>(x), (int)B, (int)H,
              (int)W, static_cast<__half*>(out));
@@ -428,7 +360,7 @@ extern "C" PFD_API int pfd_mlsd_dw_f16(const void* x, int32_t B, int32_t H, int3
     return set_error("pfd_mlsd_dw_f16: x, w and out must be 16-byte aligned");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long work = (long long)B * (H / stride) * (W / stride) * (C / 8);
-  const int g = grid_cap_m(work, 256);
+  const int g = grid_cap(work, 256);
   if (stride == 1)
     launch_k(mlsd_dw_kernel<1>, dim3(g), dim3(256), (size_t)0, st, static_cast<const __half*>(x), (int)B, (int)H,
              (int)W, (int)C, w, b, static_cast<__half*>(out));
@@ -444,7 +376,7 @@ extern "C" PFD_API int pfd_mlsd_upsample_f16(const void* x, int32_t B, int32_t h
     return set_error("pfd_mlsd_upsample_f16: bad arguments (B=%d h=%d w=%d C=%d pitch=%lld)", B, h, w, C,
                      (long long)pitch);
   if (misaligned(x) || misaligned(out)) return set_error("pfd_mlsd_upsample_f16: x and out must be 16-byte aligned");
-  const int g = grid_cap_m((long long)B * 4 * h * w * (C / 8), 256);
+  const int g = grid_cap((long long)B * 4 * h * w * (C / 8), 256);
   launch_k(mlsd_upsample_kernel, dim3(g), dim3(256), (size_t)0, static_cast<cudaStream_t>(stream),
            static_cast<const __half*>(x), (int)B, (int)h, (int)w, (int)C, static_cast<__half*>(out), (long long)pitch);
   return check_launch("mlsd_upsample");
@@ -455,7 +387,7 @@ extern "C" PFD_API int pfd_mlsd_head_f32(const void* x, int32_t B, int32_t h, in
   if (!x || !wt || !b || !out || B <= 0 || h <= 0 || w <= 0 || C <= 0 || C % 8 || C > 256)
     return set_error("pfd_mlsd_head_f32: bad arguments (B=%d h=%d w=%d C=%d)", B, h, w, C);
   if (misaligned(x)) return set_error("pfd_mlsd_head_f32: x must be 16-byte aligned");
-  launch_k(mlsd_head_kernel, dim3(grid_cap_m((long long)B * h * w, 128)), dim3(128), (size_t)5 * C * sizeof(float),
+  launch_k(mlsd_head_kernel, dim3(grid_cap((long long)B * h * w, 128)), dim3(128), (size_t)5 * C * sizeof(float),
            static_cast<cudaStream_t>(stream), static_cast<const __half*>(x), (int)B, (int)h, (int)w, (int)C, wt, b, out);
   return check_launch("mlsd_head");
 }
@@ -465,7 +397,7 @@ extern "C" PFD_API int pfd_mlsd_decode_f32(const float* maps, int32_t B, int32_t
   if (!maps || !keys || !segs || !count || B <= 0 || h <= 0 || w <= 0 || (long long)h * w < MLSD_TOPK)
     return set_error("pfd_mlsd_decode_f32: bad arguments (B=%d h=%d w=%d; h*w must be >= %d)", B, h, w, MLSD_TOPK);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  launch_k(mlsd_nms_kernel, dim3(grid_cap_m((long long)B * h * w, 256)), dim3(256), (size_t)0, st, maps, (int)B,
+  launch_k(mlsd_nms_kernel, dim3(grid_cap((long long)B * h * w, 256)), dim3(256), (size_t)0, st, maps, (int)B,
            (int)h, (int)w, thr_v, keys);
   if (int rc = check_launch("mlsd_nms")) return rc;
   launch_k(mlsd_select_kernel, dim3(B), dim3(SEL_THREADS), (size_t)0, st, static_cast<const uint32_t*>(keys), maps,

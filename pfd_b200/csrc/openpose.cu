@@ -31,6 +31,7 @@
 
 #include "../../include/pfd_b200.h"
 #include "common.h"
+#include "cvdraw.cuh"
 
 namespace pfd {
 
@@ -39,18 +40,6 @@ constexpr int OP_ROWS = PFD_OPENPOSE_MAX_PERSONS;
 constexpr int OP_PRIMS = 35;          // per person: 17 limbs, then 18 keypoints
 constexpr int OP_CIN = 16;            // network input channels: b, g, r and 13 zero pads (the GEMM's 3x3 path)
 constexpr int OP_RADIUS = 12;         // int(4.0 * 3 + 0.5)
-
-__device__ __forceinline__ void pdl_enter_o() {
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-}
-
-static inline int grid_cap_o(long long work, int per_block) {
-  long long g = (work + per_block - 1) / per_block;
-  const long long cap = (long long)num_sms() * 16;
-  if (g > cap) g = cap;
-  return (int)(g < 1 ? 1 : g);
-}
 
 // limbSeq (1-based parts) and mapIdx (PAF channels + 19) of body.py:115-121
 __constant__ int8_t c_limb_a[19] = {2, 2, 3, 4, 6, 7, 2, 9, 10, 2, 12, 13, 2, 1, 15, 1, 16, 3, 6};
@@ -75,7 +64,7 @@ template <typename T>
 __global__ void __launch_bounds__(256)
 op_input_kernel(const T* __restrict__ x, int B, int H, int W, int h, int w, int hp, int wp, int mode, int fy, int fx,
                 OpAxis ay, OpAxis ax, __half* __restrict__ out) {
-  pdl_enter_o();
+  pdl_enter();
   const long long total = (long long)B * hp * wp;
   const long long hw = (long long)H * W;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -136,7 +125,7 @@ op_input_kernel(const T* __restrict__ x, int B, int H, int W, int h, int w, int 
 
 __global__ void __launch_bounds__(256)
 op_pool_kernel(const __half* __restrict__ x, int B, int H, int W, int C, __half* __restrict__ out) {
-  pdl_enter_o();
+  pdl_enter();
   const int Ho = H / 2, Wo = W / 2, V = C / 8;
   const long long total = (long long)B * Ho * Wo * V;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -164,7 +153,7 @@ op_pool_kernel(const __half* __restrict__ x, int B, int H, int W, int C, __half*
 // out[(n*H + y)*W + x][tap * C + c] = x[n, y + tap/7 - 3, x + tap%7 - 3, c] (0 outside); one thread per 8 channels
 __global__ void __launch_bounds__(256)
 op_im2col7_kernel(const __half* __restrict__ x, int B, int H, int W, int C, __half* __restrict__ out) {
-  pdl_enter_o();
+  pdl_enter();
   const int V = C / 8;
   const long long total = (long long)B * H * W * 49 * V;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
@@ -187,7 +176,7 @@ op_im2col7_kernel(const __half* __restrict__ x, int B, int H, int W, int C, __ha
 __global__ void __launch_bounds__(256)
 op_head_kernel(const __half* __restrict__ x, int B, int h, int w, int C, const float* __restrict__ wt,
                const float* __restrict__ bias, int N, int relu, float* __restrict__ out, int out_c, int out_off) {
-  pdl_enter_o();
+  pdl_enter();
   const long long hw = (long long)h * w, total = (long long)B * hw * N;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const long long p = i % (B * hw);
@@ -235,7 +224,7 @@ __device__ __forceinline__ float op_resample(const float* __restrict__ s, int ws
 __global__ void __launch_bounds__(256)
 op_resize_kernel(const float* __restrict__ src, int B, int src_c, int c0, int C, int hs, int ws, int H, int W, int mode,
                  int fy, int fx, OpAxis ay, OpAxis ax, float* __restrict__ out) {
-  pdl_enter_o();
+  pdl_enter();
   const long long HW = (long long)H * W, total = (long long)B * C * HW;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int X = (int)(i % W);
@@ -260,7 +249,7 @@ template <typename TI>
 __global__ void __launch_bounds__(256)
 op_gauss_kernel(const TI* __restrict__ in, long long planes, int H, int W, int axis, const double* __restrict__ g,
                 double* __restrict__ out) {
-  pdl_enter_o();
+  pdl_enter();
   const long long HW = (long long)H * W, total = planes * HW;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int X = (int)(i % W);
@@ -294,7 +283,7 @@ __device__ __forceinline__ bool op_is_peak(const double* __restrict__ m, int H, 
 // one warp per (image, part, row): rowcnt[plane * H + y] = number of peaks in the row
 __global__ void __launch_bounds__(256)
 op_peak_count_kernel(const double* __restrict__ blur, long long planes, int H, int W, int* __restrict__ rowcnt) {
-  pdl_enter_o();
+  pdl_enter();
   const long long row = (long long)blockIdx.x * 8 + threadIdx.x / 32;
   const int lane = threadIdx.x & 31;
   if (row >= planes * H) return;
@@ -314,7 +303,7 @@ __global__ void __launch_bounds__(256)
 op_peak_emit_kernel(const double* __restrict__ blur, const float* __restrict__ maps, long long planes, int H, int W,
                     const int* __restrict__ rowcnt, int* __restrict__ xy, double* __restrict__ score,
                     int* __restrict__ total) {
-  pdl_enter_o();
+  pdl_enter();
   const long long row = (long long)blockIdx.x * 8 + threadIdx.x / 32;
   const int lane = threadIdx.x & 31;
   if (row >= planes * H) return;
@@ -348,7 +337,7 @@ __device__ __forceinline__ int op_round(double v) { return (int)rint(v); }
 __global__ void __launch_bounds__(256)
 op_paf_kernel(const float* __restrict__ up, int up_c, int hs, int ws, int H, int W, int mode, int fy, int fx, OpAxis ay,
               OpAxis ax, const int* __restrict__ total, const int* __restrict__ xy, double* __restrict__ conn) {
-  pdl_enter_o();
+  pdl_enter();
   const int n = blockIdx.z, k = blockIdx.y;
   const int pair = blockIdx.x * blockDim.x + threadIdx.x;
   if (pair >= OP_CAP * OP_CAP) return;
@@ -402,7 +391,7 @@ op_assemble_kernel(const int* __restrict__ total, const double* __restrict__ sco
   __shared__ int s_conn_i[OP_CAP], s_conn_j[OP_CAP];
   __shared__ double s_conn_s[OP_CAP];
   __shared__ int s_nconn, s_nrows;
-  pdl_enter_o();
+  pdl_enter();
   const int n = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   if (tid == 0) {
     int b = 0;
@@ -544,62 +533,6 @@ __device__ __forceinline__ void op_put(int* idx, int H, int W, long long x, long
   if (x >= 0 && x < W && y >= 0 && y < H) atomicMax(idx + y * W + x, prim);
 }
 
-// OpenCV's clipLine(Size(W, H), pt1, pt2) in int64 (drawing.cpp): false when the segment misses the image
-__device__ bool op_clip(long long W, long long H, long long& x1, long long& y1, long long& x2, long long& y2) {
-  const long long right = W - 1, bottom = H - 1;
-  int c1 = (x1 < 0) + (x1 > right) * 2 + (y1 < 0) * 4 + (y1 > bottom) * 8;
-  int c2 = (x2 < 0) + (x2 > right) * 2 + (y2 < 0) * 4 + (y2 > bottom) * 8;
-  if ((c1 & c2) == 0 && (c1 | c2) != 0) {
-    long long a;
-    if (c1 & 12) {
-      a = c1 < 8 ? 0 : bottom;
-      x1 += (long long)__ddiv_rn(__dmul_rn((double)(a - y1), (double)(x2 - x1)), (double)(y2 - y1));
-      y1 = a;
-      c1 = (x1 < 0) + (x1 > right) * 2;
-    }
-    if (c2 & 12) {
-      a = c2 < 8 ? 0 : bottom;
-      x2 += (long long)__ddiv_rn(__dmul_rn((double)(a - y2), (double)(x2 - x1)), (double)(y2 - y1));
-      y2 = a;
-      c2 = (x2 < 0) + (x2 > right) * 2;
-    }
-    if ((c1 & c2) == 0 && (c1 | c2) != 0) {
-      if (c1) {
-        a = c1 == 1 ? 0 : right;
-        y1 += (long long)__ddiv_rn(__dmul_rn((double)(a - x1), (double)(y2 - y1)), (double)(x2 - x1));
-        x1 = a;
-        c1 = 0;
-      }
-      if (c2) {
-        a = c2 == 1 ? 0 : right;
-        y2 += (long long)__ddiv_rn(__dmul_rn((double)(a - x2), (double)(y2 - y1)), (double)(x2 - x1));
-        x2 = a;
-        c2 = 0;
-      }
-    }
-  }
-  return (c1 | c2) == 0;
-}
-
-// cv2.line(..., 1, LINE_8) pixels, warp-parallel: clipLine, then the 8-connected LineIterator in closed form
-__device__ void op_line(int* idx, int H, int W, long long x1, long long y1, long long x2, long long y2, int prim,
-                        int lane) {
-  if (!op_clip(W, H, x1, y1, x2, y2)) return;
-  if (x2 < x1) {
-    long long t = x1; x1 = x2; x2 = t;
-    t = y1; y1 = y2; y2 = t;
-  }
-  const long long dx = x2 - x1, ady = y2 >= y1 ? y2 - y1 : y1 - y2;
-  const long long sy = y2 >= y1 ? 1 : -1;
-  const bool vert = ady > dx;
-  const long long D = vert ? ady : dx, d = vert ? dx : ady;
-  for (long long i = lane; i <= D; i += 32) {
-    const long long a = 2 * d * i - D;
-    const long long m = D == 0 ? 0 : (a >= 0 ? (a + 2 * D - 1) / (2 * D) : -((-a) / (2 * D)));
-    op_put(idx, H, W, vert ? x1 + m : x1 + i, vert ? y1 + sy * i : y1 + sy * m, prim);
-  }
-}
-
 constexpr int OP_WARPS = 4;
 constexpr int OP_DRAW_BLOCKS = 64;   // per image: 256 warps share the primitives
 
@@ -698,7 +631,8 @@ __device__ void op_draw_prim(const int* __restrict__ persons, const int* __restr
   // fillConvexPoly(shift 0, LINE_8): the outline as lines, then spans between the two edge walkers
   for (int i = 0; i < np; ++i) {
     const int a = i == 0 ? np - 1 : i - 1;
-    op_line(canvas, H, W, pts[a][0], pts[a][1], pts[i][0], pts[i][1], prim, lane);
+    for_each_line_pixel(W, H, pts[a][0], pts[a][1], pts[i][0], pts[i][1], lane,
+                        [&](long long x, long long y) { atomicMax(canvas + y * W + x, prim); });
   }
   long long xmin = pts[0][0], xmax = pts[0][0], ymin = pts[0][1], ymax = pts[0][1];
   int imin = 0;
@@ -758,7 +692,7 @@ __global__ void __launch_bounds__(OP_WARPS * 32)
 op_draw_kernel(const int* __restrict__ persons, const int* __restrict__ npersons, const int* __restrict__ xy, int H,
                int W, const float* __restrict__ sintab, int* __restrict__ idx) {
   __shared__ int s_pts[OP_WARPS][362][2];
-  pdl_enter_o();
+  pdl_enter();
   const int n = blockIdx.y, warp = threadIdx.x / 32, lane = threadIdx.x & 31;
   const int nprim = npersons[n] * OP_PRIMS;
   for (int prim = blockIdx.x * OP_WARPS + warp; prim < nprim; prim += gridDim.x * OP_WARPS)
@@ -769,7 +703,7 @@ op_draw_kernel(const int* __restrict__ persons, const int* __restrict__ npersons
 __global__ void __launch_bounds__(256)
 op_color_kernel(const int* __restrict__ idx, int B, int H, int W, const unsigned char* __restrict__ colors,
                 float* __restrict__ out) {
-  pdl_enter_o();
+  pdl_enter();
   const long long HW = (long long)H * W, total = (long long)B * HW;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int v = idx[i];
@@ -784,7 +718,6 @@ op_color_kernel(const int* __restrict__ idx, int B, int H, int W, const unsigned
 
 using namespace pfd;
 
-static bool misaligned_o(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
 
 static bool axis_ok(const int32_t* idx, const void* w, int32_t taps) { return idx && w && taps > 0; }
 
@@ -797,10 +730,10 @@ extern "C" PFD_API int pfd_openpose_input_f16(const void* x, int32_t x_f32, int3
       (mode >= 2 && (!axis_ok(iy, wy, ty) || !axis_ok(ix, wx, tx) || (mode == 2 && (ty != 8 || tx != 8)))) ||
       (mode == 0 && (h != H || w != W)))
     return set_error("pfd_openpose_input_f16: bad arguments (B=%d H=%d W=%d h=%d w=%d mode=%d)", B, H, W, h, w, mode);
-  if (misaligned_o(out)) return set_error("pfd_openpose_input_f16: out must be 16-byte aligned");
+  if (misaligned(out)) return set_error("pfd_openpose_input_f16: out must be 16-byte aligned");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const OpAxis ay{iy, wy, ty}, ax{ix, wx, tx};
-  const int g = grid_cap_o((long long)B * hp * wp, 256);
+  const int g = grid_cap((long long)B * hp * wp, 256);
   if (x_f32)
     launch_k(op_input_kernel<float>, dim3(g), dim3(256), (size_t)0, st, static_cast<const float*>(x), (int)B, (int)H,
              (int)W, (int)h, (int)w, (int)hp, (int)wp, (int)mode, (int)fy, (int)fx, ay, ax, static_cast<__half*>(out));
@@ -814,8 +747,8 @@ extern "C" PFD_API int pfd_openpose_pool_f16(const void* x, int32_t B, int32_t H
                                              void* stream) {
   if (!x || !out || B <= 0 || H < 2 || W < 2 || C <= 0 || C % 8)
     return set_error("pfd_openpose_pool_f16: bad arguments (B=%d H=%d W=%d C=%d)", B, H, W, C);
-  if (misaligned_o(x) || misaligned_o(out)) return set_error("pfd_openpose_pool_f16: x and out must be 16-byte aligned");
-  launch_k(op_pool_kernel, dim3(grid_cap_o((long long)B * (H / 2) * (W / 2) * (C / 8), 256)), dim3(256), (size_t)0,
+  if (misaligned(x) || misaligned(out)) return set_error("pfd_openpose_pool_f16: x and out must be 16-byte aligned");
+  launch_k(op_pool_kernel, dim3(grid_cap((long long)B * (H / 2) * (W / 2) * (C / 8), 256)), dim3(256), (size_t)0,
            static_cast<cudaStream_t>(stream), static_cast<const __half*>(x), (int)B, (int)H, (int)W, (int)C,
            static_cast<__half*>(out));
   return check_launch("openpose_pool");
@@ -825,8 +758,8 @@ extern "C" PFD_API int pfd_im2col7x7_f16(const void* x, int32_t B, int32_t H, in
                                          void* stream) {
   if (!x || !out || B <= 0 || H <= 0 || W <= 0 || C <= 0 || C % 8)
     return set_error("pfd_im2col7x7_f16: bad arguments (B=%d H=%d W=%d C=%d)", B, H, W, C);
-  if (misaligned_o(x) || misaligned_o(out)) return set_error("pfd_im2col7x7_f16: x and out must be 16-byte aligned");
-  launch_k(op_im2col7_kernel, dim3(grid_cap_o((long long)B * H * W * 49 * (C / 8), 256)), dim3(256), (size_t)0,
+  if (misaligned(x) || misaligned(out)) return set_error("pfd_im2col7x7_f16: x and out must be 16-byte aligned");
+  launch_k(op_im2col7_kernel, dim3(grid_cap((long long)B * H * W * 49 * (C / 8), 256)), dim3(256), (size_t)0,
            static_cast<cudaStream_t>(stream), static_cast<const __half*>(x), (int)B, (int)H, (int)W, (int)C,
            static_cast<__half*>(out));
   return check_launch("im2col7x7");
@@ -838,8 +771,8 @@ extern "C" PFD_API int pfd_openpose_head_f32(const void* x, int32_t B, int32_t h
   if (!x || !wt || !b || !out || B <= 0 || h <= 0 || w <= 0 || C <= 0 || C % 8 || N <= 0 || out_off < 0 ||
       out_off + N > out_c)
     return set_error("pfd_openpose_head_f32: bad arguments (B=%d h=%d w=%d C=%d N=%d)", B, h, w, C, N);
-  if (misaligned_o(x)) return set_error("pfd_openpose_head_f32: x must be 16-byte aligned");
-  launch_k(op_head_kernel, dim3(grid_cap_o((long long)B * h * w * N, 256)), dim3(256), (size_t)0,
+  if (misaligned(x)) return set_error("pfd_openpose_head_f32: x must be 16-byte aligned");
+  launch_k(op_head_kernel, dim3(grid_cap((long long)B * h * w * N, 256)), dim3(256), (size_t)0,
            static_cast<cudaStream_t>(stream), static_cast<const __half*>(x), (int)B, (int)h, (int)w, (int)C, wt, b,
            (int)N, (int)relu, out, (int)out_c, (int)out_off);
   return check_launch("openpose_head");
@@ -856,7 +789,7 @@ extern "C" PFD_API int pfd_openpose_resize_f32(const float* src, int32_t B, int3
     return set_error("pfd_openpose_resize_f32: bad arguments (B=%d C=%d %dx%d -> %dx%d mode=%d)", B, C, hs, ws, H, W,
                      mode);
   const OpAxis ay{iy, wy, ty}, ax{ix, wx, tx};
-  launch_k(op_resize_kernel, dim3(grid_cap_o((long long)B * C * H * W, 256)), dim3(256), (size_t)0,
+  launch_k(op_resize_kernel, dim3(grid_cap((long long)B * C * H * W, 256)), dim3(256), (size_t)0,
            static_cast<cudaStream_t>(stream), src, (int)B, (int)src_c, (int)c0, (int)C, (int)hs, (int)ws, (int)H,
            (int)W, (int)mode, (int)fy, (int)fx, ay, ax, out);
   return check_launch("openpose_resize");
@@ -869,10 +802,10 @@ extern "C" PFD_API int pfd_openpose_peaks_f32(const float* maps, int32_t B, int3
     return set_error("pfd_openpose_peaks_f32: bad arguments (B=%d H=%d W=%d)", B, H, W);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long planes = (long long)B * 18, px = planes * H * W;
-  launch_k(op_gauss_kernel<float>, dim3(grid_cap_o(px, 256)), dim3(256), (size_t)0, st, maps, planes, (int)H, (int)W,
+  launch_k(op_gauss_kernel<float>, dim3(grid_cap(px, 256)), dim3(256), (size_t)0, st, maps, planes, (int)H, (int)W,
            0, gauss, tmp);
   if (int rc = check_launch("openpose_gauss_y")) return rc;
-  launch_k(op_gauss_kernel<double>, dim3(grid_cap_o(px, 256)), dim3(256), (size_t)0, st,
+  launch_k(op_gauss_kernel<double>, dim3(grid_cap(px, 256)), dim3(256), (size_t)0, st,
            static_cast<const double*>(tmp), planes, (int)H, (int)W, 1, gauss, blur);
   if (int rc = check_launch("openpose_gauss_x")) return rc;
   const long long rowsn = planes * H;
@@ -917,7 +850,7 @@ extern "C" PFD_API int pfd_openpose_draw_f32(const int32_t* persons, const int32
            static_cast<const int*>(persons), static_cast<const int*>(npersons), static_cast<const int*>(xy), (int)H,
            (int)W, sintab, static_cast<int*>(idx));
   if (int rc = check_launch("openpose_draw")) return rc;
-  launch_k(op_color_kernel, dim3(grid_cap_o((long long)B * H * W, 256)), dim3(256), (size_t)0, st,
+  launch_k(op_color_kernel, dim3(grid_cap((long long)B * H * W, 256)), dim3(256), (size_t)0, st,
            static_cast<const int*>(idx), (int)B, (int)H, (int)W, static_cast<const unsigned char*>(colors), out);
   return check_launch("openpose_color");
 }

@@ -25,18 +25,6 @@
 
 namespace pfd {
 
-__device__ __forceinline__ void pdl_enter_p() {
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-}
-
-static inline int grid_cap_p(long long work, int per_block) {
-  long long g = (work + per_block - 1) / per_block;
-  const long long cap = (long long)num_sms() * 16;
-  if (g > cap) g = cap;
-  return (int)(g < 1 ? 1 : g);
-}
-
 __device__ __forceinline__ uint4 hmax4(uint4 a, uint4 b) {
   uint4 r;
   const __half2* x = reinterpret_cast<const __half2*>(&a);
@@ -54,7 +42,7 @@ template <int KS, bool POOL>
 __global__ void __launch_bounds__(256)
 pidinet_dw_kernel(const __half* __restrict__ x, int B, int Hin, int Win, int C, const float* __restrict__ wt,
                   __half* __restrict__ out, __half* __restrict__ pooled) {
-  pdl_enter_p();
+  pdl_enter();
   const int h = POOL ? Hin / 2 : Hin, w = POOL ? Win / 2 : Win;
   const int V = C / 8;
   const long long total = (long long)B * h * w * V;
@@ -120,7 +108,7 @@ __global__ void __launch_bounds__(128)
 pidinet_reduce_kernel(const __half* __restrict__ x, long long P, int C, const float* __restrict__ wg,
                       const float* __restrict__ bg, __half* __restrict__ m) {
   extern __shared__ float s_w[];
-  pdl_enter_p();
+  pdl_enter();
   for (int i = threadIdx.x; i < C * PIDI_D; i += blockDim.x) s_w[i] = wg[i];
   __syncthreads();
   for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; p < P; p += (long long)gridDim.x * blockDim.x) {
@@ -189,7 +177,7 @@ pidinet_cdcm_kernel(const __half* __restrict__ m, int h, int w, const uint2* __r
   uint4* s_tile = reinterpret_cast<uint4*>(cd_smem);
   const uint32_t* s_tw = reinterpret_cast<const uint32_t*>(cd_smem);
   uint2* s_b = reinterpret_cast<uint2*>(cd_smem + CD_SMEM_TILE);
-  pdl_enter_p();
+  pdl_enter();
   const int n = blockIdx.z, ty0 = blockIdx.y * CD_T, tx0 = blockIdx.x * CD_T;
   for (int i = threadIdx.x; i < CD_STEPS * 3 * 32; i += CD_THREADS) s_b[i] = __ldg(wpk + i);
   const __half* mn = m + (long long)n * h * w * PIDI_D;
@@ -258,7 +246,7 @@ __global__ void __launch_bounds__(256)
 pidinet_side_kernel(const float* __restrict__ u, int B, int h, int w, const float* __restrict__ prm,
                     float* __restrict__ side) {
   __shared__ float s_p[PFD_PIDINET_SIDE_PARAMS];
-  pdl_enter_p();
+  pdl_enter();
   for (int i = threadIdx.x; i < PFD_PIDINET_SIDE_PARAMS; i += blockDim.x) s_p[i] = prm[i];
   __syncthreads();
   const float* w1 = s_p;
@@ -342,7 +330,7 @@ __device__ __forceinline__ float resize_bilinear_pt(const float* __restrict__ s,
 
 __global__ void pidinet_fuse_kernel(PidiSides sd, int B, int H, int W, const float* __restrict__ cls,
                                     float* __restrict__ out) {
-  pdl_enter_p();
+  pdl_enter();
   const double c0 = cls[0], c1 = cls[1], c2 = cls[2], c3 = cls[3], cb = cls[4];
   const long long hw = (long long)H * W;
   const long long total = (long long)B * hw;
@@ -375,12 +363,11 @@ extern "C" PFD_API int pfd_pidinet_dw_f16(const void* x, int32_t B, int32_t Hin,
   if (!x || !w || !out || B <= 0 || Hin <= 0 || Win <= 0 || C <= 0 || C % 8 || (ks != 3 && ks != 5) ||
       (pool && (!pooled || ks != 3 || Hin < 2 || Win < 2)))
     return set_error("pfd_pidinet_dw_f16: bad arguments (B=%d H=%d W=%d C=%d ks=%d pool=%d)", B, Hin, Win, C, ks, pool);
-  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(pooled) |
-       reinterpret_cast<uintptr_t>(w)) & 15)
+  if (misaligned(x) || misaligned(out) || misaligned(pooled) || misaligned(w))
     return set_error("pfd_pidinet_dw_f16: x, w, out and pooled must be 16-byte aligned");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long work = (long long)B * (pool ? Hin / 2 : Hin) * (pool ? Win / 2 : Win) * (C / 8);
-  const int g = grid_cap_p(work, 256);
+  const int g = grid_cap(work, 256);
   const __half* xi = static_cast<const __half*>(x);
   __half* o = static_cast<__half*>(out);
   __half* p = static_cast<__half*>(pooled);
@@ -400,9 +387,9 @@ extern "C" PFD_API int pfd_pidinet_reduce_f16(const void* x, int64_t P, int32_t 
                                               void* m, void* stream) {
   if (!x || !w || !b || !m || P <= 0 || C <= 0 || C % 8 || C > 512)
     return set_error("pfd_pidinet_reduce_f16: bad arguments (P=%lld C=%d)", (long long)P, C);
-  if ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(m)) & 15)
+  if (misaligned(x) || misaligned(m))
     return set_error("pfd_pidinet_reduce_f16: x and m must be 16-byte aligned");
-  launch_k(pidinet_reduce_kernel, dim3(grid_cap_p(P, 128)), dim3(128), (size_t)C * PIDI_D * sizeof(float),
+  launch_k(pidinet_reduce_kernel, dim3(grid_cap(P, 128)), dim3(128), (size_t)C * PIDI_D * sizeof(float),
            static_cast<cudaStream_t>(stream), static_cast<const __half*>(x), (long long)P, (int)C, w, b,
            static_cast<__half*>(m));
   return check_launch("pidinet_reduce");
@@ -412,7 +399,7 @@ extern "C" PFD_API int pfd_pidinet_cdcm_f16(const void* m, int32_t B, int32_t h,
                                             void* stream) {
   if (!m || !wpk || !u || B <= 0 || h <= 0 || w <= 0 || B > 65535)
     return set_error("pfd_pidinet_cdcm_f16: bad arguments (B=%d h=%d w=%d)", B, h, w);
-  if ((reinterpret_cast<uintptr_t>(m) | reinterpret_cast<uintptr_t>(wpk) | reinterpret_cast<uintptr_t>(u)) & 15)
+  if (misaligned(m) || misaligned(wpk) || misaligned(u))
     return set_error("pfd_pidinet_cdcm_f16: m, wpk and u must be 16-byte aligned");
   static bool attr_done = false;
   if (!attr_done) {
@@ -430,8 +417,8 @@ extern "C" PFD_API int pfd_pidinet_side_f32(const float* u, int32_t B, int32_t h
                                             float* side, void* stream) {
   if (!u || !params || !side || B <= 0 || h <= 0 || w <= 0)
     return set_error("pfd_pidinet_side_f32: bad arguments (B=%d h=%d w=%d)", B, h, w);
-  if (reinterpret_cast<uintptr_t>(u) & 15) return set_error("pfd_pidinet_side_f32: u must be 16-byte aligned");
-  launch_k(pidinet_side_kernel, dim3(grid_cap_p((long long)B * h * w, 256)), dim3(256), (size_t)0,
+  if (misaligned(u)) return set_error("pfd_pidinet_side_f32: u must be 16-byte aligned");
+  launch_k(pidinet_side_kernel, dim3(grid_cap((long long)B * h * w, 256)), dim3(256), (size_t)0,
            static_cast<cudaStream_t>(stream), u, (int)B, (int)h, (int)w, params, side);
   return check_launch("pidinet_side");
 }
@@ -451,7 +438,7 @@ extern "C" PFD_API int pfd_pidinet_fuse_f32(const float* const* sides, const int
     sd.sy[k] = (float)side_h[k] / (float)H;
     sd.sx[k] = (float)side_w[k] / (float)W;
   }
-  launch_k(pidinet_fuse_kernel, dim3(grid_cap_p((long long)B * H * W, 256)), dim3(256), (size_t)0,
+  launch_k(pidinet_fuse_kernel, dim3(grid_cap((long long)B * H * W, 256)), dim3(256), (size_t)0,
            static_cast<cudaStream_t>(stream), sd, (int)B, (int)H, (int)W, cls, out);
   return check_launch("pidinet_fuse");
 }

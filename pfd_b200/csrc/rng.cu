@@ -38,8 +38,7 @@ __device__ __forceinline__ float2 box_muller(uint32_t wa, uint32_t wb) {
 
 __global__ void randn_f16_kernel(__half* __restrict__ out, int B, long long n, const unsigned long long* __restrict__ seeds,
                                  uint32_t stream_id, int draw, const int* __restrict__ draw_dev, float scale) {
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  pdl_enter();
   const uint32_t d = (uint32_t)(draw + (draw_dev ? *draw_dev : 0));
   const long long groups = (n + 3) / 4;
   const long long items = groups * B;
@@ -74,10 +73,7 @@ extern "C" PFD_API int pfd_randn_f16(void* out, int32_t B, int64_t n, const uint
                                      int32_t draw, const int32_t* draw_dev, float scale, void* stream) {
   if (!out || !seeds || B <= 0 || n <= 0) return set_error("pfd_randn_f16: null/empty argument");
   const long long items = ((long long)n + 3) / 4 * B;
-  long long g = (items + 255) / 256;
-  const long long cap = (long long)num_sms() * 16;
-  if (g > cap) g = cap;
-  launch_k(randn_f16_kernel, dim3((unsigned)g), dim3(256), (size_t)0, static_cast<cudaStream_t>(stream),
+  launch_k(randn_f16_kernel, dim3(grid_cap(items, 256)), dim3(256), (size_t)0, static_cast<cudaStream_t>(stream),
            static_cast<__half*>(out), (int)B, (long long)n, reinterpret_cast<const unsigned long long*>(seeds),
            stream_id, (int)draw, reinterpret_cast<const int*>(draw_dev), scale);
   return check_launch("randn_f16");

@@ -25,11 +25,6 @@
 
 namespace pfd {
 
-__device__ __forceinline__ void pdl_enter_s() {
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-}
-
 // cv2.borderInterpolate(BORDER_REFLECT_101): ... 2 1 | 0 1 2 ... n-1 | n-2 ..., folded until inside
 __device__ __forceinline__ int reflect101(int i, int n) {
   if (n == 1) return 0;
@@ -56,7 +51,7 @@ scribble_nms_kernel(const float* __restrict__ hed, long long img_stride, int H, 
   __shared__ float s_in[IN][IN];
   __shared__ float s_row[IN][G];
   __shared__ float s_g[G][G + 1];
-  pdl_enter_s();
+  pdl_enter();
   const int n = blockIdx.z;
   const int x0 = blockIdx.x * ST, y0 = blockIdx.y * ST;
   const float* src = hed + (long long)n * img_stride;
@@ -108,7 +103,7 @@ scribble_blur_u8_kernel(const unsigned char* __restrict__ z, int H, int W, Fixed
   constexpr int IN = ST + 2 * SU_R;
   __shared__ int s_in[IN][IN];
   __shared__ int s_row[IN][ST];
-  pdl_enter_s();
+  pdl_enter();
   const int n = blockIdx.z;
   const int x0 = blockIdx.x * ST, y0 = blockIdx.y * ST;
   const unsigned char* src = z + (long long)n * H * W;
@@ -159,7 +154,7 @@ scribble_xdog_kernel(const T* __restrict__ x, int H, int W, int threshold, Taps5
   __shared__ unsigned char s_in[3][IN][IN];
   __shared__ float s_r2[IN][ST];
   __shared__ float s_r1[IN1][ST];
-  pdl_enter_s();
+  pdl_enter();
   const int n = blockIdx.z;
   const int x0 = blockIdx.x * ST, y0 = blockIdx.y * ST;
   const long long hw = (long long)H * W;

@@ -27,7 +27,8 @@ import torch
 import torch.nn as nn
 
 from . import native as nv
-from .modules import Conv2d, IndexedSequential, cached, pack_conv3x3, pad_cols
+from .annotator import AnnotatorNetwork
+from .modules import Conv2d, IndexedSequential, cached, pack_conv, pad_cols
 
 SCALE = 1.0 / 255.0
 # hed/__init__.py:16,64,105: pretrained/controlnet/preprocess/hed/ControlNetHED.pth relative to the working directory
@@ -68,7 +69,7 @@ class ControlNetHED(nn.Module):
             for bi, blk in enumerate(self.blocks()):
                 layer = []
                 for ci, conv in enumerate(blk.convs):
-                    w = pack_conv3x3(conv.weight)
+                    w = pack_conv(conv.weight)
                     if bi == 0 and ci == 0:
                         w = pad_cols(w)                                   # K = 27 -> 32 for the im2col GEMM
                     b = (conv.bias.detach().float() * SCALE).to(torch.float16).contiguous()
@@ -106,37 +107,11 @@ class ControlNetHED(nn.Module):
         return (out, sides) if return_sides else out
 
 
-_network: Optional[ControlNetHED] = None
-
-
-def set_network(m: Optional[ControlNetHED]) -> None:
-    """Install the process-wide HED network (or None to drop it)."""
-    global _network
-    _network = m
-
-
-def load_hed(path: Optional[str] = None) -> ControlNetHED:
-    """Read ControlNetHED.pth (default: the reference's location relative to the working directory) with
-    strict=True and install it.  Raises FileNotFoundError when the file is absent; never downloads."""
-    path = path or DEFAULT_PATH
-    if not os.path.isfile(path):
-        raise FileNotFoundError(f"HED annotator weights not found: {path}")
-    sd = torch.load(path, map_location="cpu", weights_only=True)
-    m = ControlNetHED()
-    m.load_state_dict(sd, strict=True)
-    m.eval()
-    set_network(m)
-    return m
-
-
-def get_network() -> ControlNetHED:
-    """The installed network, loading it from DEFAULT_PATH on first use."""
-    return _network if _network is not None else load_hed()
+_network: Optional[ControlNetHED] = None  # set through NETWORK.set (set_network)
+NETWORK = AnnotatorNetwork(__name__, ControlNetHED, DEFAULT_PATH, "HED annotator")
+set_network, load_hed, get_network = NETWORK.set, NETWORK.load, NETWORK.get
 
 
 def preprocess_hed(x: torch.Tensor) -> torch.Tensor:
     """ControlNet.preprocess(x, type='hed') for a CUDA [B,3,H,W] image in [0,1] -> float32 [B,3,H,W]."""
-    net = get_network()
-    if net.norm.device != x.device:
-        net.to(x.device)                                       # apply_hed: netNetwork.to(device) (:111)
-    return net.apply(x)
+    return NETWORK.on(x).apply(x)                              # apply_hed: netNetwork.to(device) (:111)

@@ -41,7 +41,8 @@ import torch
 import torch.nn as nn
 
 from . import native as nv
-from .modules import cached
+from .annotator import AnnotatorNetwork
+from .modules import cached, fp16, pack_conv
 
 # mlsd/__init__.py:11-16,59: pretrained/controlnet/preprocess/mlsd/mlsd_large_512_fp32.pth relative to the working
 # directory
@@ -142,38 +143,14 @@ def fold_bn(conv: nn.Module, bn: nn.Module):
     return f(conv.weight) * scale.reshape(-1, 1, 1, 1), (b - f(bn.running_mean)) * scale + f(bn.bias)
 
 
-def _gemm_w(w: torch.Tensor, cin: Optional[int] = None) -> torch.Tensor:
-    """[N, C, k, k] fp32 -> the GEMM's fp16 [N, k*k*C] (k = tap * C + c), input channels zero-padded to cin."""
-    n, c, kh, kw = w.shape
-    if cin is not None and cin > c:
-        w = torch.cat([w, w.new_zeros((n, cin - c, kh, kw))], 1)
-    return w.permute(0, 2, 3, 1).reshape(n, -1).to(torch.float16).contiguous()
-
-
-def _h(b: torch.Tensor) -> torch.Tensor:
-    return b.to(torch.float16).contiguous()
-
-
-def _conv1x1_into(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, out: torch.Tensor, act: int) -> None:
-    """act(1x1 conv of x [B,H,W,C] + b) written into out, a [B,H,W,N] view with unit channel stride."""
-    B, H, W, C = x.shape
-    nv.gemm_raw([(x, 1, C, (x.stride(2), x.stride(1), x.stride(0)))], in_w=W, in_h=H, stride=1, W=W, H=H, NB=B, w=w,
-                N=w.shape[0], K=w.stride(0), act=act, bias=b, out=out,
-                so=(out.stride(0), 0, out.stride(1), out.stride(2), 0, 1))
-
-
 def _dilated5(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
     """relu(conv3x3(x, dilation 5, padding 5) + b) of x [B,h,w,C]: phase (p, q) of the output only reads phase (p, q)
     of the input, with a plain 3x3 / padding 1 conv, so each phase is one GEMM on strided views."""
-    B, h, wd, C = x.shape
+    B, h, wd, _ = x.shape
     out = torch.empty((B, h, wd, w.shape[0]), device=x.device, dtype=torch.float16)
     for p in range(min(5, h)):
         for q in range(min(5, wd)):
-            a, o = x[:, p::5, q::5], out[:, p::5, q::5]
-            hs, ws = a.shape[1], a.shape[2]
-            nv.gemm_raw([(a, 9, C, (a.stride(2), a.stride(1), a.stride(0)))], in_w=ws, in_h=hs, stride=1, W=ws, H=hs,
-                        NB=B, w=w, N=w.shape[0], K=w.stride(0), act=nv.ACT_RELU, bias=b, out=o,
-                        so=(o.stride(0), 0, o.stride(1), o.stride(2), 0, 1))
+            nv.conv3x3(x[:, p::5, q::5], w, b, act=nv.ACT_RELU, out=out[:, p::5, q::5])
     return out
 
 
@@ -198,26 +175,26 @@ class MLSD(nn.Module):
                 raise RuntimeError("MLSD.apply needs the network on a CUDA device (call .to('cuda'))")
             f = self.backbone.features
             w, b = fold_bn(f[0][0], f[0][1])
-            stem = (_gemm_w(w / 127.5, STEM_CIN), _h(b))           # the input arrives as u8 - 127.5 (exact levels)
+            stem = (pack_conv(w / 127.5, STEM_CIN), fp16(b))      # the input arrives as u8 - 127.5 (exact levels)
             trunk = []
             for i, inp, hid, oup, stride, res in trunk_layers():
                 seq = f[i].conv
                 expand = None
                 if hid != inp:
                     w, b = fold_bn(seq[0][0], seq[0][1])
-                    expand = (_gemm_w(w), _h(b))
+                    expand = (pack_conv(w), fp16(b))
                     seq = seq[1:]
                 w, b = fold_bn(seq[0][0], seq[0][1])
                 dw = (w.reshape(hid, 9).t().contiguous(), b.contiguous())
                 w, b = fold_bn(seq[1], seq[2])
-                trunk.append((i, stride, res, expand, dw, (_gemm_w(w), _h(b))))
+                trunk.append((i, stride, res, expand, dw, (pack_conv(w), fp16(b))))
             decoder = []
             for k, (name, _, _, up) in enumerate(DECODER):
                 ba, bb = getattr(self, name), getattr(self, f"block{16 + 2 * k}")
                 convs = [fold_bn(s[0], s[1]) for s in (ba.conv1, ba.conv2, bb.conv1, bb.conv2)]
-                decoder.append((up, *[(_gemm_w(w), _h(b)) for w, b in convs]))
+                decoder.append((up, *[(pack_conv(w), fp16(b)) for w, b in convs]))
             c = self.block23
-            dil, conv2 = [(_gemm_w(w), _h(b)) for w, b in (fold_bn(c.conv1[0], c.conv1[1]),
+            dil, conv2 = [(pack_conv(w), fp16(b)) for w, b in (fold_bn(c.conv1[0], c.conv1[1]),
                                                             fold_bn(c.conv2[0], c.conv2[1]))]
             head = (c.conv3.weight.detach().float()[KEEP].reshape(5, -1).contiguous(),
                     c.conv3.bias.detach().float()[KEEP].contiguous())
@@ -241,11 +218,11 @@ class MLSD(nn.Module):
         for (up, (w1, b1), (w2, b2), (wb1, bb1), (wb2, bb2)), a in zip(decoder, feats[3::-1]):
             B, hh, ww, _ = a.shape
             cat = torch.empty((B, hh, ww, 128), device=a.device, dtype=torch.float16)
-            _conv1x1_into(a, w2, b2, cat[..., :64], nv.ACT_RELU)
+            nv.conv1x1_into(a, w2, b2, cat[..., :64], act=nv.ACT_RELU)
             if up:
                 nv.mlsd_upsample(nv.conv1x1(x, w1, b1, act=nv.ACT_RELU), cat[..., 64:])
             else:
-                _conv1x1_into(x, w1, b1, cat[..., 64:], nv.ACT_RELU)
+                nv.conv1x1_into(x, w1, b1, cat[..., 64:], act=nv.ACT_RELU)
             t = nv.conv3x3(cat, wb1, bb1, act=nv.ACT_RELU, residual=cat)
             x = nv.conv3x3(t, wb2, bb2, act=nv.ACT_RELU)
         x = nv.conv3x3(_dilated5(x, *dil), *conv2, act=nv.ACT_RELU)
@@ -271,48 +248,9 @@ class MLSD(nn.Module):
         return (out, {"maps": maps, "segs": segs, "count": count}) if debug else out
 
 
-_network: Optional[MLSD] = None
-
-
-def set_network(m: Optional[MLSD]) -> None:
-    """Install the process-wide M-LSD network (or None to drop it)."""
-    global _network
-    _network = m
-
-
-def _read_state_dict(path: str):
-    """A .safetensors file, or a torch file (read with weights_only=True) with or without a top-level 'state_dict';
-    'module.' is removed from the keys."""
-    if os.path.splitext(path)[1].lower() == ".safetensors":
-        import safetensors.torch
-        sd = safetensors.torch.load_file(path, device="cpu")
-    else:
-        sd = torch.load(path, map_location="cpu", weights_only=True)
-    sd = sd.get("state_dict", sd)
-    return {k.replace("module.", ""): v for k, v in sd.items()}
-
-
-def load_mlsd(path: Optional[str] = None) -> MLSD:
-    """Read mlsd_large_512_fp32.pth (default: the reference's location relative to the working directory) with
-    strict=True and install it.  Raises FileNotFoundError when the file is absent; never downloads."""
-    path = path or DEFAULT_PATH
-    if not os.path.isfile(path):
-        raise FileNotFoundError(f"M-LSD annotator weights not found: {path}")
-    m = MLSD()
-    m.load_state_dict(_read_state_dict(path), strict=True)
-    m.eval()
-    set_network(m)
-    return m
-
-
-def available() -> bool:
-    """True when a network is installed or the default checkpoint exists (so get_network() can load it)."""
-    return _network is not None or os.path.isfile(DEFAULT_PATH)
-
-
-def get_network() -> MLSD:
-    """The installed network, loading it from DEFAULT_PATH on first use."""
-    return _network if _network is not None else load_mlsd()
+_network: Optional[MLSD] = None  # set through NETWORK.set (set_network)
+NETWORK = AnnotatorNetwork(__name__, MLSD, DEFAULT_PATH, "M-LSD annotator")
+set_network, load_mlsd, get_network, available = NETWORK.set, NETWORK.load, NETWORK.get, NETWORK.available
 
 
 def preprocess_mlsd(x: torch.Tensor, thr_v: float = 0.1, thr_d: float = 0.1) -> torch.Tensor:
@@ -322,7 +260,4 @@ def preprocess_mlsd(x: torch.Tensor, thr_v: float = 0.1, thr_d: float = 0.1) -> 
             "controlnet annotator 'mlsd' needs the M-LSD weights, which are not installed: put "
             f"mlsd_large_512_fp32.pth at {DEFAULT_PATH}, call pfd_b200.mlsd.load_mlsd(path) or "
             "pfd_b200.mlsd.set_network(net), or feed a ready control map (do_preprocess=False)")
-    net = get_network()
-    if net.block23.conv3.weight.device != x.device:
-        net.to(x.device)                                       # apply_mlsd: mlsdmodel.to(device) (:67)
-    return net.apply(x, thr_v, thr_d)
+    return NETWORK.on(x).apply(x, thr_v, thr_d)                # apply_mlsd: mlsdmodel.to(device) (:67)

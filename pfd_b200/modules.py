@@ -76,7 +76,8 @@ def cached(mod: nn.Module, key: str, params: Sequence[Optional[torch.Tensor]], f
     return hit[1]
 
 
-def _h(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+def fp16(t: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
+    """A contiguous fp16 copy of a parameter (None stays None); the network must be on a CUDA device."""
     if t is None:
         return None
     if not t.is_cuda:
@@ -101,19 +102,23 @@ def pad_cols(w: torch.Tensor, mult: int = 8) -> torch.Tensor:
     return torch.cat([w, pad], 1).contiguous()
 
 
-def pack_conv3x3(weight: torch.Tensor) -> torch.Tensor:
-    """[O, I, 3, 3] -> [O, 9*I] with k = tap*I + c (tap = ky*3 + kx), the K order of pfd_gemm_f16."""
-    o, i = weight.shape[:2]
-    return _h(weight).permute(0, 2, 3, 1).reshape(o, 9 * i).contiguous()
+def pack_conv(weight: torch.Tensor, cin: Optional[int] = None) -> torch.Tensor:
+    """[O, I, k, k] -> fp16 [O, k*k*C] with K = tap*C + c (tap = ky*k + kx), the K order of pfd_gemm_f16; the input
+    channels are zero-padded to C = cin when cin > I."""
+    w = fp16(weight)
+    o, i, kh, kw = w.shape
+    if cin is not None and cin > i:
+        w = torch.cat([w, w.new_zeros((o, cin - i, kh, kw))], 1)
+    return w.permute(0, 2, 3, 1).reshape(o, -1).contiguous()
 
 
 def pk_conv3(conv: nn.Conv2d, skip: Optional[nn.Conv2d] = None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
     """Packed 3x3 weights (+ optional fused 1x1 skip conv appended along K, biases summed)."""
     def build():
-        w = pack_conv3x3(conv.weight)
-        b = _h(conv.bias)
+        w = pack_conv(conv.weight)
+        b = fp16(conv.bias)
         if skip is not None:
-            ws = _h(skip.weight).reshape(skip.weight.shape[0], -1)
+            ws = fp16(skip.weight).reshape(skip.weight.shape[0], -1)
             w = torch.cat([w, ws], 1).contiguous()
             if skip.bias is not None:
                 b = (conv.bias.detach().float() + skip.bias.detach().float()).to(torch.float16).contiguous()
@@ -128,8 +133,8 @@ def pk_conv3(conv: nn.Conv2d, skip: Optional[nn.Conv2d] = None) -> Tuple[torch.T
 def pk_conv3_small(conv: nn.Conv2d) -> Tuple[torch.Tensor, Optional[torch.Tensor], int]:
     """3x3 conv with tiny Cin (im2col path): weights [O, Kpad], Kpad = ceil8(9*Cin)."""
     def build():
-        w = pad_cols(pack_conv3x3(conv.weight))
-        b = _h(conv.bias)
+        w = pad_cols(pack_conv(conv.weight))
+        b = fp16(conv.bias)
         if w.shape[0] % 8:
             w, b = pad_rows(w), (pad_rows(b) if b is not None else None)
         return w, b, w.shape[1]
@@ -140,8 +145,8 @@ def pk_mat(mod: nn.Module, weight: torch.Tensor, bias: Optional[torch.Tensor], k
            rows: Optional[slice] = None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
     """Linear / 1x1-conv weights as [N, K] fp16 (optionally a row slice, e.g. one third of in_proj)."""
     def build():
-        w = _h(weight).reshape(weight.shape[0], -1)
-        b = _h(bias)
+        w = fp16(weight).reshape(weight.shape[0], -1)
+        b = fp16(bias)
         if rows is not None:
             w = w[rows].contiguous()
             b = b[rows].contiguous() if b is not None else None
@@ -158,8 +163,8 @@ def pk_lin(lin: nn.Module, key: str = "mat"):
 
 
 def pk_norm(norm: nn.Module) -> Tuple[torch.Tensor, torch.Tensor]:
-    return cached(norm, "norm", [norm.weight, norm.bias], lambda: (_h(norm.weight), _h(norm.bias)))
+    return cached(norm, "norm", [norm.weight, norm.bias], lambda: (fp16(norm.weight), fp16(norm.bias)))
 
 
 def pk_vec(mod: nn.Module, t: torch.Tensor, key: str) -> torch.Tensor:
-    return cached(mod, key, [t], lambda: _h(t))
+    return cached(mod, key, [t], lambda: fp16(t))

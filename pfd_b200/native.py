@@ -252,6 +252,19 @@ def _chk16(t: torch.Tensor, name: str) -> None:
         raise RuntimeError(f"{name}: expected a CUDA fp16 tensor, got {t.dtype} on {t.device}")
 
 
+def _chk32(t: torch.Tensor, name: str) -> None:
+    if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
+        raise RuntimeError(f"{name}: expected a contiguous CUDA fp32 tensor, got {t.dtype} on {t.device}")
+
+
+def _chk_image(x: torch.Tensor, what: str) -> Tuple[torch.Tensor, int]:
+    """An NCHW [B,3,H,W] CUDA fp16/fp32 image -> (x contiguous, 1 if it is fp32 else 0)."""
+    if x.dim() != 4 or x.shape[1] != 3 or not x.is_cuda or x.dtype not in (torch.float16, torch.float32):
+        raise RuntimeError(f"{what}: expected a CUDA fp16/fp32 [B,3,H,W] image, got {tuple(x.shape)} {x.dtype} "
+                           f"{x.device}")
+    return x.contiguous(), int(x.dtype == torch.float32)
+
+
 # --------------------------------------------------------------------------------------------
 # GEMM family
 # --------------------------------------------------------------------------------------------
@@ -367,6 +380,17 @@ def conv1x1(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = Non
     r = residual.reshape(NB * H * W, -1) if residual is not None else None
     linear(x.reshape(NB * H * W, C), w, bias, act=act, residual=r, out=out.reshape(NB * H * W, N),
            x2=None if x2 is None else x2.reshape(NB * H * W, -1))
+    return out
+
+
+def conv1x1_into(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], out: torch.Tensor, *,
+                 act: int = ACT_NONE) -> torch.Tensor:
+    """act(1x1 conv of x + bias) between channel-last views: x [NB,H,W,C] and out [NB,H,W,N] may have any pixel
+    strides (e.g. channel slices of concat buffers) but unit channel stride."""
+    NB, H, W, C = x.shape
+    gemm_raw([(x, 1, C, (x.stride(2), x.stride(1), x.stride(0)))], in_w=W, in_h=H, stride=1, W=W, H=H, NB=NB, w=w,
+             N=w.shape[0], K=w.stride(0), act=act, bias=bias, out=out,
+             so=(out.stride(0), 0, out.stride(1), out.stride(2), 0, 1))
     return out
 
 
@@ -632,14 +656,12 @@ def vae_posterior(moments: torch.Tensor, zc: int, *, noise: Optional[torch.Tenso
 def canny(x: torch.Tensor, low: int = 100, high: int = 200) -> Tuple[torch.Tensor, int]:
     """NCHW [B,3,H,W] image in [0,1] (fp16/fp32) -> (float32 [B,3,H,W] edge map, hysteresis sweeps).  Bit-exact
     cv2.Canny(ToPILImage(x), low, high) (pfd_canny_f32); synchronises the stream."""
-    if x.dim() != 4 or x.shape[1] != 3 or not x.is_cuda or x.dtype not in (torch.float16, torch.float32):
-        raise RuntimeError(f"canny: expected a CUDA fp16/fp32 [B,3,H,W] image, got {tuple(x.shape)} {x.dtype} {x.device}")
-    x = x.contiguous()
+    x, f32 = _chk_image(x, "canny")
     B, _, H, W = x.shape
     ws = torch.empty(int(load().pfd_canny_workspace_bytes(B, H, W)), device=x.device, dtype=torch.uint8)
     out = torch.empty((B, 3, H, W), device=x.device, dtype=torch.float32)
     sweeps = c_int32(0)
-    _check(load().pfd_canny_f32(x.data_ptr(), int(x.dtype == torch.float32), B, H, W, int(low), int(high),
+    _check(load().pfd_canny_f32(x.data_ptr(), f32, B, H, W, int(low), int(high),
                                 ws.data_ptr(), out.data_ptr(), ctypes.byref(sweeps), stream_ptr()), "pfd_canny_f32")
     return out, int(sweeps.value)
 
@@ -655,21 +677,14 @@ def image_u8_roundtrip(x: torch.Tensor) -> torch.Tensor:
     return out
 
 
-def _chk32(t: torch.Tensor, name: str) -> None:
-    if t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous():
-        raise RuntimeError(f"{name}: expected a contiguous CUDA fp32 tensor, got {t.dtype} on {t.device}")
-
-
 def hed_input(x: torch.Tensor, norm: torch.Tensor, scale: float, cpad: int = 3) -> torch.Tensor:
     """NCHW [B,3,H,W] image in [0,1] (fp16/fp32) -> channel-last fp16 [B,H,W,cpad] = (x.mul(255).byte() - norm) * scale,
     zero pad channels (pfd_hed_input_f16).  norm: CUDA fp32 [3]."""
-    if x.dim() != 4 or x.shape[1] != 3 or not x.is_cuda or x.dtype not in (torch.float16, torch.float32):
-        raise RuntimeError(f"hed_input: expected a CUDA fp16/fp32 [B,3,H,W] image, got {tuple(x.shape)} {x.dtype}")
+    x, f32 = _chk_image(x, "hed_input")
     _chk32(norm, "hed_input norm")
-    x = x.contiguous()
     B, _, H, W = x.shape
     out = torch.empty((B, H, W, cpad), device=x.device, dtype=torch.float16)
-    _check(load().pfd_hed_input_f16(x.data_ptr(), int(x.dtype == torch.float32), B, H, W, cpad, norm.data_ptr(),
+    _check(load().pfd_hed_input_f16(x.data_ptr(), f32, B, H, W, cpad, norm.data_ptr(),
                                     float(scale), out.data_ptr(), stream_ptr()), "pfd_hed_input_f16")
     return out
 
@@ -742,12 +757,10 @@ def scribble_blur_u8(z: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
 def scribble_xdog(x: torch.Tensor, threshold: int = 32) -> torch.Tensor:
     """The xdog scribble of an NCHW [B,3,H,W] image in [0,1] (fp16/fp32) -> float32 [B,3,H,W]
     (pfd_scribble_xdog_f32).  threshold: integer; the uint8 edge strength is compared with `>`."""
-    if x.dim() != 4 or x.shape[1] != 3 or not x.is_cuda or x.dtype not in (torch.float16, torch.float32):
-        raise RuntimeError(f"scribble_xdog: expected a CUDA fp16/fp32 [B,3,H,W] image, got {tuple(x.shape)} {x.dtype}")
-    x = x.contiguous()
+    x, f32 = _chk_image(x, "scribble_xdog")
     B, _, H, W = x.shape
     out = torch.empty((B, 3, H, W), device=x.device, dtype=torch.float32)
-    _check(load().pfd_scribble_xdog_f32(x.data_ptr(), int(x.dtype == torch.float32), B, H, W, int(threshold),
+    _check(load().pfd_scribble_xdog_f32(x.data_ptr(), f32, B, H, W, int(threshold),
                                         out.data_ptr(), stream_ptr()), "pfd_scribble_xdog_f32")
     return out
 
@@ -838,12 +851,10 @@ def pidinet_fuse(sides: Sequence[torch.Tensor], cls: torch.Tensor, H: int, W: in
 def mlsd_input(x: torch.Tensor) -> torch.Tensor:
     """NCHW [B,3,H,W] image in [0,1] (fp16/fp32) -> channel-last fp16 [B,H,W,16] = [u8 - 127.5 (rgb), 1 - 127.5, 0 x 12]
     with u8 = x.mul(255).byte() (pfd_mlsd_input_f16)."""
-    if x.dim() != 4 or x.shape[1] != 3 or not x.is_cuda or x.dtype not in (torch.float16, torch.float32):
-        raise RuntimeError(f"mlsd_input: expected a CUDA fp16/fp32 [B,3,H,W] image, got {tuple(x.shape)} {x.dtype}")
-    x = x.contiguous()
+    x, f32 = _chk_image(x, "mlsd_input")
     B, _, H, W = x.shape
     out = torch.empty((B, H, W, 16), device=x.device, dtype=torch.float16)
-    _check(load().pfd_mlsd_input_f16(x.data_ptr(), int(x.dtype == torch.float32), B, H, W, out.data_ptr(),
+    _check(load().pfd_mlsd_input_f16(x.data_ptr(), f32, B, H, W, out.data_ptr(),
                                      stream_ptr()), "pfd_mlsd_input_f16")
     return out
 
@@ -928,13 +939,11 @@ def openpose_input(x: torch.Tensor, h: int, w: int, hp: int, wp: int, plan, tabs
     """NCHW [B,3,H,W] image in [0,1] -> channel-last fp16 [B,hp,wp,16]: u8 = x.mul(255).byte(), BGR, cv2.resize to
     h x w by ``plan`` (openpose_tables.resize_plan; ``tabs`` its device tables), 128 pad, u8 / 256 - 0.5
     (pfd_openpose_input_f16)."""
-    if x.dim() != 4 or x.shape[1] != 3 or not x.is_cuda or x.dtype not in (torch.float16, torch.float32):
-        raise RuntimeError(f"openpose_input: expected a CUDA fp16/fp32 [B,3,H,W] image, got {tuple(x.shape)} {x.dtype}")
-    x = x.contiguous()
+    x, f32 = _chk_image(x, "openpose_input")
     B, _, H, W = x.shape
     out = torch.empty((B, hp, wp, 16), device=x.device, dtype=torch.float16)
     mode, fy, fx, ay, ax = _plan_args(plan, tabs, u8=True)
-    _check(load().pfd_openpose_input_f16(x.data_ptr(), int(x.dtype == torch.float32), B, H, W, h, w, hp, wp, mode, fy,
+    _check(load().pfd_openpose_input_f16(x.data_ptr(), f32, B, H, W, h, w, hp, wp, mode, fy,
                                          fx, *ay, *ax, out.data_ptr(), stream_ptr()), "pfd_openpose_input_f16")
     return out
 

@@ -40,7 +40,8 @@ import torch.nn as nn
 
 from . import native as nv
 from . import openpose_tables as T
-from .modules import cached
+from .annotator import AnnotatorNetwork, read_state_dict
+from .modules import cached, fp16, pack_conv
 
 # openpose/__init__.py:11,123-127: pretrained/controlnet/preprocess/openpose/body_pose_model.pth relative to the working
 # directory.  Only the body file is needed here (the reference also loads the hand and face networks).
@@ -81,15 +82,6 @@ class _Seq(nn.Module):
             setattr(self, name, _Conv(cin, cout, k))
 
 
-def _gemm_w(w: torch.Tensor, cin: Optional[int] = None) -> torch.Tensor:
-    """[N, C, k, k] -> the GEMM's fp16 [N, k*k*C] (k = tap * C + c), input channels zero-padded to cin."""
-    n, c, kh, kw = w.shape
-    w = w.detach().float()
-    if cin is not None and cin > c:
-        w = torch.cat([w, w.new_zeros((n, cin - c, kh, kw))], 1)
-    return w.permute(0, 2, 3, 1).reshape(n, -1).to(torch.float16).contiguous()
-
-
 def _cat_w(w: torch.Tensor) -> torch.Tensor:
     """A stage's first 7x7 weights [128, 185, 7, 7] with the input channels moved to the concat buffer's layout."""
     w = w.detach().float()
@@ -103,7 +95,7 @@ def _rows(w: torch.Tensor, b: torch.Tensor, n: int):
     wp = w.detach().float().new_zeros((n,) + tuple(w.shape[1:]))
     bp = b.detach().float().new_zeros((n,))
     wp[:w.shape[0]], bp[:b.shape[0]] = w.detach().float(), b.detach().float()
-    return _gemm_w(wp), bp.to(torch.float16).contiguous()
+    return pack_conv(wp), fp16(bp)
 
 
 class BodyPose(nn.Module):
@@ -126,24 +118,23 @@ class BodyPose(nn.Module):
         def build():
             if not self.model0.conv1_1.weight.is_cuda:
                 raise RuntimeError("BodyPose.apply needs the network on a CUDA device (call .to('cuda'))")
-            h = lambda b: b.detach().to(torch.float16).contiguous()                     # noqa: E731
             trunk = []
             for v in VGG:
                 if v == "pool":
                     trunk.append(None)
                     continue
                 c = getattr(self.model0, v[0])
-                trunk.append((_gemm_w(c.weight, CIN if v[1] < CIN else None), h(c.bias)))
+                trunk.append((pack_conv(c.weight, CIN if v[1] < CIN else None), fp16(c.bias)))
             stages = []
             for i in range(1, 7):
                 a, b = self._conv(i, 1, 0), self._conv(i, 2, 0)
                 wa = a.weight if i == 1 else _cat_w(a.weight)
                 wb = b.weight if i == 1 else _cat_w(b.weight)
-                first = (torch.cat([_gemm_w(wa), _gemm_w(wb)]), torch.cat([h(a.bias), h(b.bias)]))
+                first = (torch.cat([pack_conv(wa), pack_conv(wb)]), torch.cat([fp16(a.bias), fp16(b.bias)]))
                 branches = []
                 for L, pad in ((1, L1_PAD), (2, L2_PAD)):
                     n = len(_layers(i, L))
-                    mid = [(_gemm_w(self._conv(i, L, j).weight), h(self._conv(i, L, j).bias)) for j in range(1, n - 1)]
+                    mid = [(pack_conv(c.weight), fp16(c.bias)) for c in (self._conv(i, L, j) for j in range(1, n - 1))]
                     last = self._conv(i, L, n - 1)
                     if i < 6:
                         tail = _rows(last.weight, last.bias, pad)
@@ -187,10 +178,7 @@ class BodyPose(nn.Module):
             for L, ((mid, tail), t) in enumerate(zip(branches, outs)):
                 if i < 6:
                     lo = 0 if L == 0 else L1_PAD
-                    o = cat[..., lo:lo + tail[0].shape[0]]
-                    nv.gemm_raw([(t, 1, t.shape[3], (t.stride(2), t.stride(1), t.stride(0)))], in_w=w, in_h=h,
-                                stride=1, W=w, H=h, NB=B, w=tail[0], N=tail[0].shape[0], K=tail[0].stride(0),
-                                bias=tail[1], out=o, so=(o.stride(0), 0, o.stride(1), o.stride(2), 0, 1))
+                    nv.conv1x1_into(t, *tail, cat[..., lo:lo + tail[0].shape[0]])
                 else:
                     nv.openpose_head(t, tail[0], tail[1], L == 1, maps, 0 if L == 0 else 38)
         return maps
@@ -244,51 +232,19 @@ class BodyPose(nn.Module):
                      "persons": persons, "person_score": pscore, "npersons": npersons}
 
 
-_network: Optional[BodyPose] = None
-
-
-def set_network(m: Optional[BodyPose]) -> None:
-    """Install the process-wide OpenPose body network (or None to drop it)."""
-    global _network
-    _network = m
-
-
 def _read_state_dict(path: str):
-    """A .safetensors file or a torch file (weights_only=True); the raw CMU keys ('conv1_1.weight', which the
-    reference's util.transfer maps) get their block prefix back, 'module.' is removed."""
-    if os.path.splitext(path)[1].lower() == ".safetensors":
-        import safetensors.torch
-        sd = safetensors.torch.load_file(path, device="cpu")
-    else:
-        sd = torch.load(path, map_location="cpu", weights_only=True)
-    sd = {k.replace("module.", ""): v for k, v in sd.get("state_dict", sd).items()}
+    """read_state_dict, then the raw CMU keys ('conv1_1.weight', which the reference's util.transfer maps) get their
+    block prefix back."""
+    sd = read_state_dict(path)
     if not any(k.startswith("model0.") for k in sd):
         block = {name: blk for blk, seq in BodyPose().named_children() for name, _ in seq.named_children()}
         sd = {f"{block[k.rsplit('.', 1)[0]]}.{k}" if k.rsplit(".", 1)[0] in block else k: v for k, v in sd.items()}
     return sd
 
 
-def load_openpose(path: Optional[str] = None) -> BodyPose:
-    """Read body_pose_model.pth (default: the reference's location relative to the working directory) with strict=True
-    and install it.  Raises FileNotFoundError when the file is absent; never downloads."""
-    path = path or DEFAULT_PATH
-    if not os.path.isfile(path):
-        raise FileNotFoundError(f"OpenPose body weights not found: {path}")
-    m = BodyPose()
-    m.load_state_dict(_read_state_dict(path), strict=True)
-    m.eval()
-    set_network(m)
-    return m
-
-
-def available() -> bool:
-    """True when a network is installed or the default checkpoint exists (so get_network() can load it)."""
-    return _network is not None or os.path.isfile(DEFAULT_PATH)
-
-
-def get_network() -> BodyPose:
-    """The installed network, loading it from DEFAULT_PATH on first use."""
-    return _network if _network is not None else load_openpose()
+_network: Optional[BodyPose] = None  # set through NETWORK.set (set_network)
+NETWORK = AnnotatorNetwork(__name__, BodyPose, DEFAULT_PATH, "OpenPose body", read=_read_state_dict)
+set_network, load_openpose, get_network, available = NETWORK.set, NETWORK.load, NETWORK.get, NETWORK.available
 
 
 def preprocess_openpose(x: torch.Tensor) -> torch.Tensor:
@@ -298,7 +254,4 @@ def preprocess_openpose(x: torch.Tensor) -> torch.Tensor:
             "controlnet annotator 'openpose' needs the OpenPose body weights, which are not installed: put "
             f"body_pose_model.pth at {DEFAULT_PATH}, call pfd_b200.openpose.load_openpose(path) or "
             "pfd_b200.openpose.set_network(net), or feed a ready control map (do_preprocess=False)")
-    net = get_network()
-    if net.model0.conv1_1.weight.device != x.device:
-        net.to(x.device)
-    return net.apply(x)
+    return NETWORK.on(x).apply(x)

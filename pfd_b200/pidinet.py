@@ -39,6 +39,7 @@ import torch
 import torch.nn as nn
 
 from . import native as nv
+from .annotator import AnnotatorNetwork
 from .modules import cached
 
 # pidinet/__init__.py:7-11,68-71: pretrained/controlnet/preprocess/pidinet/table5_pidinet.pth relative to the working
@@ -236,53 +237,11 @@ class PiDiNet(nn.Module):
         return (out, sides) if return_sides else out
 
 
-_network: Optional[PiDiNet] = None
-
-
-def set_network(m: Optional[PiDiNet]) -> None:
-    """Install the process-wide PiDiNet network (or None to drop it)."""
-    global _network
-    _network = m
-
-
-def _read_state_dict(path: str):
-    """What the reference's load_state_dict accepts (pidinet/__init__.py:52-65): a .safetensors file, or a torch file
-    (read with weights_only=True) with or without a top-level 'state_dict'; 'module.' is removed from the keys."""
-    if os.path.splitext(path)[1].lower() == ".safetensors":
-        import safetensors.torch
-        sd = safetensors.torch.load_file(path, device="cpu")
-    else:
-        sd = torch.load(path, map_location="cpu", weights_only=True)
-    sd = sd.get("state_dict", sd)
-    return {k.replace("module.", ""): v for k, v in sd.items()}
-
-
-def load_pidinet(path: Optional[str] = None) -> PiDiNet:
-    """Read table5_pidinet.pth (default: the reference's location relative to the working directory) with strict=True
-    and install it.  Raises FileNotFoundError when the file is absent; never downloads."""
-    path = path or DEFAULT_PATH
-    if not os.path.isfile(path):
-        raise FileNotFoundError(f"PiDiNet annotator weights not found: {path}")
-    m = PiDiNet()
-    m.load_state_dict(_read_state_dict(path), strict=True)
-    m.eval()
-    set_network(m)
-    return m
-
-
-def available() -> bool:
-    """True when a network is installed or the default checkpoint exists (so get_network() can load it)."""
-    return _network is not None or os.path.isfile(DEFAULT_PATH)
-
-
-def get_network() -> PiDiNet:
-    """The installed network, loading it from DEFAULT_PATH on first use."""
-    return _network if _network is not None else load_pidinet()
+_network: Optional[PiDiNet] = None  # set through NETWORK.set (set_network)
+NETWORK = AnnotatorNetwork(__name__, PiDiNet, DEFAULT_PATH, "PiDiNet annotator")
+set_network, load_pidinet, get_network, available = NETWORK.set, NETWORK.load, NETWORK.get, NETWORK.available
 
 
 def preprocess_pidinet(x: torch.Tensor) -> torch.Tensor:
     """apply_pidinet + ToTensor + repeat for a CUDA [B,3,H,W] image in [0,1] -> float32 [B,3,H,W] (levels / 255)."""
-    net = get_network()
-    if net.classifier.weight.device != x.device:
-        net.to(x.device)                                       # apply_pidinet: netNetwork.to(device) (:80)
-    return net.apply(x)
+    return NETWORK.on(x).apply(x)                              # apply_pidinet: netNetwork.to(device) (:80)

@@ -29,7 +29,7 @@ def nv():
 
 
 def grid_cap():
-    """Elements one grid_for() launch covers in one grid-stride pass (16 CTAs of 256 threads per SM)."""
+    """Elements one grid_cap() launch covers in one grid-stride pass (16 CTAs of 256 threads per SM)."""
     return 16 * torch.cuda.get_device_properties(0).multi_processor_count * 256
 
 

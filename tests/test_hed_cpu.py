@@ -100,15 +100,21 @@ def test_load_hed_missing_file_raises_without_download(tmp_path, monkeypatch):
 def test_load_hed_strict_round_trip(tmp_path):
     from oracle.hed_oracle import synth_state_dict
     from pfd_b200 import hed
+    import safetensors.torch
     sd = synth_state_dict(3)
+    # the forms every annotator loader accepts: plain, a 'state_dict' with 'module.' keys, safetensors
+    wrapped, st = str(tmp_path / "wrapped.pth"), str(tmp_path / "ControlNetHED.safetensors")
+    torch.save({"state_dict": {"module." + k: v for k, v in sd.items()}}, wrapped)
+    safetensors.torch.save_file({k: v.contiguous() for k, v in sd.items()}, st)
     path = str(tmp_path / "ControlNetHED.pth")
     torch.save(sd, path)
     saved = hed._network
     try:
-        m = hed.load_hed(path)
-        assert hed.get_network() is m
-        for k, v in m.state_dict().items():
-            assert torch.equal(v, sd[k])
+        for p in (path, wrapped, st):
+            m = hed.load_hed(p)
+            assert hed.get_network() is m
+            for k, v in m.state_dict().items():
+                assert torch.equal(v, sd[k])
         sd.pop("norm")
         torch.save(sd, path)
         with pytest.raises(RuntimeError):
