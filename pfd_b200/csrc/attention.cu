@@ -54,11 +54,6 @@ struct FlashCfg {
   static_assert(DP % 16 == 0 && DP <= 64 * DCH, "V^T rows");
 };
 
-__device__ __forceinline__ uint32_t pack_f2h(float a, float b) {
-  const __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<const uint32_t*>(&h);
-}
-
 template <int DCH, int DP>
 __global__ void __launch_bounds__(FA_THREADS, DCH == 1 ? 2 : 1)
 flash_attn_kernel(const __grid_constant__ FlashParams p) {
@@ -209,10 +204,10 @@ flash_attn_kernel(const __grid_constant__ FlashParams p) {
       for (int r = 0; r < 4; ++r) {
         const int i = r & 1;                    // row r0 (i = 0) or r0 + 8
         const int idx = 8 * k + 4 * (r >> 1) + 2 * i;
-        const uint32_t h = pack_f2h(fast_exp2(fmaf(s[idx], c2, nm[i])), fast_exp2(fmaf(s[idx + 1], c2, nm[i])));
-        const float2 hf = __half22float2(*reinterpret_cast<const __half2*>(&h));
+        const __half2 h = __floats2half2_rn(fast_exp2(fmaf(s[idx], c2, nm[i])), fast_exp2(fmaf(s[idx + 1], c2, nm[i])));
+        const float2 hf = __half22float2(h);
         l[i] += hf.x + hf.y;
-        pa[k][r] = h;
+        pa[k][r] = *reinterpret_cast<const uint32_t*>(&h);
       }
     }
     mbar_wait(v_full(st), ph);
@@ -244,46 +239,20 @@ flash_attn_kernel(const __grid_constant__ FlashParams p) {
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
-                                  const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                  const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
+// [B, heads, rows, inner] operand at element strides (sb, sh, sr), read in boxes of 64 x box_rows
 static int encode4d(CUtensorMap* m, const void* ptr, cuuint64_t inner, cuuint64_t rows, cuuint64_t heads,
                     cuuint64_t B, long long sr, long long sh, long long sb, cuuint32_t box_rows, const char* what) {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* fp = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fp, cudaEnableDefault, &q) != cudaSuccess ||
-        q != cudaDriverEntryPointSuccess)
-      return set_error("cuTensorMapEncodeTiled entry point unavailable");
-    fn = reinterpret_cast<EncodeTiledFn>(fp);
-  }
-  cuuint64_t dims[4] = {inner, rows, heads, B};
-  cuuint64_t strides[3] = {(cuuint64_t)sr * 2, (cuuint64_t)sh * 2, (cuuint64_t)sb * 2};
-  cuuint32_t box[4] = {64, box_rows, 1, 1};
-  cuuint32_t es[4] = {1, 1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(ptr), dims, strides, box, es,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS)
-    return set_error("flash attention tensor map (%s) encode failed: CUresult %d dims[%llu,%llu,%llu,%llu] strides[%lld,%lld,%lld]",
-                     what, (int)r, (unsigned long long)inner, (unsigned long long)rows, (unsigned long long)heads,
-                     (unsigned long long)B, sr, sh, sb);
-  return 0;
+  const cuuint64_t dims[4] = {inner, rows, heads, B};
+  const cuuint64_t strides[3] = {(cuuint64_t)sr * 2, (cuuint64_t)sh * 2, (cuuint64_t)sb * 2};
+  const cuuint32_t box[4] = {64, box_rows, 1, 1};
+  const cuuint32_t es[4] = {1, 1, 1, 1};
+  return encode_tensor_map_f16(m, ptr, 4, dims, strides, box, es, what);
 }
 
 template <int DCH, int DP>
 static int launch_flash(const FlashParams& p, dim3 grid, cudaStream_t st) {
   using Cfg = FlashCfg<DCH, DP>;
-  static bool done = false;
-  if (!done) {
-    cudaError_t e = cudaFuncSetAttribute(flash_attn_kernel<DCH, DP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_BYTES);
-    if (e != cudaSuccess) return set_error("cudaFuncSetAttribute(flash d<=%d): %s", DP, cudaGetErrorString(e));
-    done = true;
-  }
+  if (int rc = smem_opt_in<flash_attn_kernel<DCH, DP>>(Cfg::SMEM_BYTES, "flash_attn_kernel")) return rc;
   launch_k(flash_attn_kernel<DCH, DP>, grid, dim3(FA_THREADS), (size_t)Cfg::SMEM_BYTES, st, p);
   return check_launch("pfd_flash_attn_f16");
 }

@@ -1,5 +1,7 @@
-// Shared helpers for the C-ABI translation units (error text, launch counter, launch geometry, kernel entry).
+// Shared helpers for the C-ABI translation units (error text, launch counter, launch geometry, kernel entry,
+// shared-memory opt-in, tensor maps, per-device scratch).
 #pragma once
+#include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -101,6 +103,34 @@ inline int grid_cap(long long work, int per_block) {
 }
 
 inline bool misaligned(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) != 0; }
+
+// Lets `kernel` use `bytes` of dynamic shared memory (beyond the default 48 KiB), once per process.  The flag is per
+// kernel instance: the kernel is a template argument, not a function pointer, whose type template instances share.
+template <auto kernel>
+inline int smem_opt_in(int bytes, const char* what) {
+  static bool done = false;
+  if (done) return 0;
+  const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  if (e != cudaSuccess) return set_error("cudaFuncSetAttribute(%s, %d bytes): %s", what, bytes, cudaGetErrorString(e));
+  done = true;
+  return 0;
+}
+
+// fp16 TMA tensor map of rank 3 or 4 with 128-byte swizzle and 256-byte L2 promotion; elements outside `dims` read as
+// zero.  dims, box and elem_strides have `rank` entries, strides_bytes rank - 1.  `what` names the operand in the error.
+int encode_tensor_map_f16(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims,
+                          const cuuint64_t* strides_bytes, const cuuint32_t* box, const cuuint32_t* elem_strides,
+                          const char* what);
+
+// Per-device scratch buffers.  Each slot holds one buffer per device, allocated by the first call on that device and
+// then shared by every later call, eager or captured, so a graph replay makes the same choices as the eager run.
+// cudaMalloc is illegal inside a stream capture: the first call must be eager (every graph-captured path of the
+// package runs eagerly first).  The launches of one device are stream-ordered by the callers (one request at a time),
+// so one buffer per device is enough.
+enum ScratchSlot { SCRATCH_SPLITK, SCRATCH_GN_DET, SCRATCH_SLOTS };
+// The slot's buffer for the current device: `bytes` long, the first `zero_bytes` zeroed when it is allocated.  Null
+// when it cannot be allocated, or when it is not allocated yet and `st` is capturing; the caller reports the error.
+void* device_scratch(ScratchSlot slot, size_t bytes, size_t zero_bytes, cudaStream_t st);
 
 // Deterministic mode (pfd_set_option "deterministic"; default from PFD_DETERMINISTIC=1 at load, see api.cu): every
 // summation order depends only on a sample's own shapes, never on the batch, the SM count or a race between CTAs.

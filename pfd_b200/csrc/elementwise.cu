@@ -7,8 +7,6 @@
 #include <cuda_runtime.h>
 #include <math.h>
 
-#include <mutex>
-
 #include "../../include/pfd_b200.h"
 #include "common.h"
 
@@ -83,6 +81,39 @@ __device__ __forceinline__ void gn_pivots(const __half* __restrict__ x1, int c1,
   }
 }
 
+// One thread's per-channel sums of d = x - K_g (sm) and of d^2 (sq) for the 8 channels from c, over the pixels pix,
+// pix + step, ... below p1 of image n, added in pixel order with LOADS loads in flight.  Both statistics kernels
+// accumulate through it, so the per-thread sums of the default and the deterministic mode are the same.  The wide-row
+// paths keep one load in flight: with four, their loop over channel vectors would not fit in 64 registers.
+template <int LOADS>
+__device__ __forceinline__ void gn_accumulate(const __half* __restrict__ x1, int c1, const __half* __restrict__ x2,
+                                              int c2, long long HW, int n, int cpg, int c, long long pix, long long p1,
+                                              int step, float (&sm)[8], float (&sq)[8]) {
+  float kp[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) sm[i] = sq[i] = 0.f;
+  gn_pivots(x1, c1, x2, c2, HW, n, cpg, c, kp);
+  const long long base = (long long)n * HW;
+  auto add = [&](const uint4& u) {
+    float f[8];
+    unpack8(u, f);
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      const float d = f[i] - kp[i];
+      sm[i] += d;
+      sq[i] += d * d;
+    }
+  };
+  for (; pix + (LOADS - 1) * step < p1; pix += LOADS * step) {
+    uint4 u[LOADS];
+#pragma unroll
+    for (int k = 0; k < LOADS; ++k) u[k] = gn_load(x1, c1, x2, c2, base + pix + k * step, c);
+#pragma unroll
+    for (int k = 0; k < LOADS; ++k) add(u[k]);
+  }
+  for (; pix < p1; pix += step) add(gn_load(x1, c1, x2, c2, base + pix, c));
+}
+
 // fold a thread's 8 per-channel sums into (at most eight) group bins, then one shared atomic per bin
 __device__ __forceinline__ void gn_fold_bins(const float (&sm)[8], const float (&sq)[8], int c, int cpg, float* s_sum,
                                              float* s_sq) {
@@ -127,58 +158,16 @@ gn_stats_kernel(const __half* __restrict__ x1, int c1, const __half* __restrict_
   if (lanes >= 1) {
     const int v = threadIdx.x % vecs;
     const int c = v * 8;
-    float sm[8], sq[8], kp[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) sm[i] = sq[i] = 0.f;
-    gn_pivots(x1, c1, x2, c2, HW, n, cpg, c, kp);
-    long long pix = p0 + threadIdx.x / vecs;
-    for (; pix + 3 * lanes < p1; pix += 4 * lanes) {
-      uint4 u[4];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) u[k] = gn_load(x1, c1, x2, c2, (long long)n * HW + pix + k * lanes, c);
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        float f[8];
-        unpack8(u[k], f);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float d = f[i] - kp[i];
-          sm[i] += d;
-          sq[i] += d * d;
-        }
-      }
-    }
-    for (; pix < p1; pix += lanes) {
-      float f[8];
-      unpack8(gn_load(x1, c1, x2, c2, (long long)n * HW + pix, c), f);
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const float d = f[i] - kp[i];
-        sm[i] += d;
-        sq[i] += d * d;
-      }
-    }
+    float sm[8], sq[8];
+    gn_accumulate<4>(x1, c1, x2, c2, HW, n, cpg, c, p0 + threadIdx.x / vecs, p1, lanes, sm, sq);
     gn_fold_bins(sm, sq, c, cpg, s_sum, s_sq);
   } else {
     // very wide rows (vecs > blockDim): a thread owns vectors v, v + blockDim, ... and walks the chunk for each, so
     // its sums stay per-thread in registers as on the narrow path (not one shared fp32 sum of the whole chunk)
     for (int v = threadIdx.x; v < vecs; v += blockDim.x) {
-      const int c = v * 8;
-      float sm[8], sq[8], kp[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) sm[i] = sq[i] = 0.f;
-      gn_pivots(x1, c1, x2, c2, HW, n, cpg, c, kp);
-      for (long long pix = p0; pix < p1; ++pix) {
-        float f[8];
-        unpack8(gn_load(x1, c1, x2, c2, (long long)n * HW + pix, c), f);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float d = f[i] - kp[i];
-          sm[i] += d;
-          sq[i] += d * d;
-        }
-      }
-      gn_fold_bins(sm, sq, c, cpg, s_sum, s_sq);
+      float sm[8], sq[8];
+      gn_accumulate<1>(x1, c1, x2, c2, HW, n, cpg, v * 8, p0, p1, 1, sm, sq);
+      gn_fold_bins(sm, sq, v * 8, cpg, s_sum, s_sq);
     }
   }
   __syncthreads();
@@ -188,7 +177,7 @@ gn_stats_kernel(const __half* __restrict__ x1, int c1, const __half* __restrict_
   }
 }
 
-// Deterministic statistics (deterministic mode).  Same per-thread accumulation as gn_stats_kernel; then
+// Deterministic statistics (deterministic mode).  The per-thread accumulation of gn_stats_kernel (gn_accumulate); then
 //   1. every thread stores its 8 per-channel fp32 sums in shared memory, red[lane][channel];
 //   2. warp w folds group g (g = w, w + warps, ...): lane l adds items l, l + 32, ... of the group's (lane, channel)
 //      list in fp64, then a fixed xor butterfly -> one fp64 (sum, sumsq) partial per (image, group, chunk) in part;
@@ -223,42 +212,12 @@ gn_stats_det_kernel(const __half* __restrict__ x1, int c1, const __half* __restr
   const int nl = lanes >= 1 ? lanes : 1;
   float* red_s = red;
   float* red_q = red + (long long)nl * C;
-  const long long base = (long long)n * HW;
   if (lanes >= 1) {
     if (threadIdx.x < lanes * vecs) {
       const int v = threadIdx.x % vecs, lane = threadIdx.x / vecs;
       const int c = v * 8;
-      float sm[8], sq[8], kp[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) sm[i] = sq[i] = 0.f;
-      gn_pivots(x1, c1, x2, c2, HW, n, cpg, c, kp);
-      long long pix = p0 + lane;
-      for (; pix + 3 * lanes < p1; pix += 4 * lanes) {
-        uint4 u[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) u[k] = gn_load(x1, c1, x2, c2, base + pix + k * lanes, c);
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-          float f[8];
-          unpack8(u[k], f);
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float d = f[i] - kp[i];
-            sm[i] += d;
-            sq[i] += d * d;
-          }
-        }
-      }
-      for (; pix < p1; pix += lanes) {
-        float f[8];
-        unpack8(gn_load(x1, c1, x2, c2, base + pix, c), f);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float d = f[i] - kp[i];
-          sm[i] += d;
-          sq[i] += d * d;
-        }
-      }
+      float sm[8], sq[8];
+      gn_accumulate<4>(x1, c1, x2, c2, HW, n, cpg, c, p0 + lane, p1, lanes, sm, sq);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         red_s[lane * C + c + i] = sm[i];
@@ -269,20 +228,8 @@ gn_stats_det_kernel(const __half* __restrict__ x1, int c1, const __half* __restr
     // very wide rows (vecs > blockDim): a thread owns vectors v, v + blockDim, ... and walks the chunk for each
     for (int v = threadIdx.x; v < vecs; v += blockDim.x) {
       const int c = v * 8;
-      float sm[8], sq[8], kp[8];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) sm[i] = sq[i] = 0.f;
-      gn_pivots(x1, c1, x2, c2, HW, n, cpg, c, kp);
-      for (long long pix = p0; pix < p1; ++pix) {
-        float f[8];
-        unpack8(gn_load(x1, c1, x2, c2, base + pix, c), f);
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const float d = f[i] - kp[i];
-          sm[i] += d;
-          sq[i] += d * d;
-        }
-      }
+      float sm[8], sq[8];
+      gn_accumulate<1>(x1, c1, x2, c2, HW, n, cpg, c, p0, p1, 1, sm, sq);
 #pragma unroll
       for (int i = 0; i < 8; ++i) {
         red_s[c + i] = sm[i];
@@ -836,42 +783,12 @@ __global__ void patchify_kernel(const T* __restrict__ x, int B, int C, int H, in
   }
 }
 
-// Scratch of the deterministic GroupNorm statistics, one per device: GN_DET_MAX_NB arrival counters, then the fp64
-// partials [NB][groups][chunks].  Allocated (and the counters zeroed) by the first deterministic call on the device,
-// which must not be inside a stream capture - every graph-captured path of the package runs eagerly first.  The
-// counters return to zero at the end of every call, and the calls of one device are stream-ordered (like the GEMM's
-// split-K workspace), so one buffer serves them all.
+// Scratch of the deterministic GroupNorm statistics (device_scratch): GN_DET_MAX_NB arrival counters, zeroed when it is
+// allocated, then the fp64 partials [NB][groups][chunks].  The counters return to zero at the end of every call.
 constexpr size_t GN_DET_COUNTER_BYTES = 256;
 constexpr size_t GN_DET_SCRATCH_BYTES =
     GN_DET_COUNTER_BYTES + sizeof(double) * 2 * GN_DET_MAX_NB * GN_MAX_GROUPS * GN_DET_MAX_CHUNKS;
 static_assert(GN_DET_MAX_NB * sizeof(int) <= GN_DET_COUNTER_BYTES, "arrival counters overflow their slot");
-
-static char* gn_det_scratch(cudaStream_t st) {
-  constexpr int MAX_DEV = 64;
-  static std::mutex mu;
-  static char* buf[MAX_DEV] = {nullptr};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= MAX_DEV) return nullptr;
-  std::lock_guard<std::mutex> lk(mu);
-  if (buf[dev]) return buf[dev];
-  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-  if (cudaStreamIsCapturing(st, &cs) != cudaSuccess || cs != cudaStreamCaptureStatusNone) {
-    (void)cudaGetLastError();
-    return nullptr;
-  }
-  char* p = nullptr;
-  if (cudaMalloc(&p, GN_DET_SCRATCH_BYTES) != cudaSuccess) {
-    (void)cudaGetLastError();
-    return nullptr;
-  }
-  if (cudaMemset(p, 0, GN_DET_COUNTER_BYTES) != cudaSuccess || cudaDeviceSynchronize() != cudaSuccess) {
-    (void)cudaGetLastError();
-    cudaFree(p);
-    return nullptr;
-  }
-  buf[dev] = p;
-  return p;
-}
 
 }  // namespace pfd
 
@@ -913,7 +830,7 @@ extern "C" PFD_API int pfd_groupnorm_f16(const void* x1, int32_t c1, const void*
     if (NB > GN_DET_MAX_NB || smem > 48 * 1024)
       return set_error("pfd_groupnorm_f16: deterministic statistics support NB <= %d and C <= 6144 (NB=%d, C=%d)",
                        GN_DET_MAX_NB, NB, C);
-    char* dscr = gn_det_scratch(st);
+    char* dscr = static_cast<char*>(device_scratch(SCRATCH_GN_DET, GN_DET_SCRATCH_BYTES, GN_DET_COUNTER_BYTES, st));
     if (!dscr) return set_error("pfd_groupnorm_f16: deterministic statistics scratch unavailable (the first "
                                 "deterministic call on a device must not be inside a stream capture)");
     launch_k(gn_stats_det_kernel, grid, dim3(threads), smem, st, static_cast<const __half*>(x1), (int)c1,
@@ -963,11 +880,7 @@ extern "C" PFD_API int pfd_softmax_f16(void* s, int64_t batch, int32_t rows, int
   if (nheads <= 0) nheads = 1;
   if (nwin <= 0) nwin = 1;
   int threads = cols >= 1024 ? 256 : (cols >= 256 ? 128 : 64);
-  static bool attr = false;
-  if (!attr) {
-    cudaFuncSetAttribute(softmax_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 50176 * 4);
-    attr = true;
-  }
+  if (int rc = smem_opt_in<softmax_rows_kernel>(50176 * 4, "softmax_rows_kernel")) return rc;
   launch_k(softmax_rows_kernel, dim3((unsigned)nrows), dim3(threads), (size_t)(cols * sizeof(float)), st, 
       static_cast<__half*>(s), batch, rows, cols, ld, scale, static_cast<const __half*>(bias), nheads,
       static_cast<const __half*>(mask), nwin);

@@ -18,8 +18,6 @@
 #include <math.h>
 #include <string.h>
 
-#include <mutex>
-
 #include "../../include/pfd_b200.h"
 #include "common.h"
 #include "ptx.cuh"
@@ -130,35 +128,38 @@ __device__ __forceinline__ float act_apply(float v, int act) {
   return v;
 }
 
-__device__ __forceinline__ void unpack8h(const uint4& u, float (&f)[8]) {
-  const __half2* h = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    float2 t = __half22float2(h[i]);
-    f[2 * i] = t.x;
-    f[2 * i + 1] = t.y;
-  }
-}
-
-__device__ __forceinline__ void load8h(const __half* p, float (&f)[8]) {
-  uint4 u = __ldg(reinterpret_cast<const uint4*>(p));
-  const __half2* h = reinterpret_cast<const __half2*>(&u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    float2 t = __half22float2(h[i]);
-    f[2 * i] = t.x;
-    f[2 * i + 1] = t.y;
-  }
-}
-
-__device__ __forceinline__ uint32_t pack_h2(float a, float b) {
-  __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-
 __device__ __forceinline__ float h2lo(uint32_t u) { return __low2float(*reinterpret_cast<const __half2*>(&u)); }
 __device__ __forceinline__ float h2hi(uint32_t u) { return __high2float(*reinterpret_cast<const __half2*>(&u)); }
 __device__ __forceinline__ uint32_t ldg_h2(const __half* p) { return __ldg(reinterpret_cast<const unsigned int*>(p)); }
+
+// The epilogue arithmetic of every output path (staged tile, direct epilogue, split-K finish).  Each path rounds these
+// values to fp16 before it adds the residual in fp16.
+//
+// act(acc * alpha + bias [+ row add]) of an adjacent column pair (lo, hi), in fp32.  The per-image row add (time
+// embedding) comes after the bias and before the activation, the reference's (conv + bias) + emb -> act.
+// bias and ra hold the fp16 pairs of the bias and the row add.
+__device__ __forceinline__ void epi_pair(float& lo, float& hi, float alpha, uint32_t bias, bool rowadd, uint32_t ra,
+                                         int act) {
+  lo = fmaf(lo, alpha, h2lo(bias));
+  hi = fmaf(hi, alpha, h2hi(bias));
+  if (rowadd) {
+    lo += h2lo(ra);
+    hi += h2hi(ra);
+  }
+  if (act != PFD_ACT_NONE) {
+    lo = act_apply(lo, act);
+    hi = act_apply(hi, act);
+  }
+}
+
+// GEGLU output pair fp16(value) * fp16(gelu(fp16(gate))), value and gate each acc * alpha + bias.  The reference's
+// x, gate = proj(x).chunk(2) are fp16 tensors, and it computes x * gelu(gate) in fp16 (attention.py:50-51).
+// bv and bg hold the fp16 bias pairs of value and gate.
+__device__ __forceinline__ __half2 geglu_pair(const float* v, const float* g, float alpha, uint32_t bv, uint32_t bg) {
+  const __half2 a = __floats2half2_rn(fmaf(v[0], alpha, h2lo(bv)), fmaf(v[1], alpha, h2hi(bv)));
+  const float2 gf = __half22float2(__floats2half2_rn(fmaf(g[0], alpha, h2lo(bg)), fmaf(g[1], alpha, h2hi(bg))));
+  return __hmul2(a, __floats2half2_rn(gelu_sig(gf.x), gelu_sig(gf.y)));
+}
 
 // One unit of work of a persistent CTA: K blocks [kb0, kb1) of output tile `tile`, the whole contraction of the tile
 // or, with split-K, slice `slot`.
@@ -264,12 +265,7 @@ __device__ __forceinline__ void gemm_stage_tile(const GemmParams& p, const float
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         if (!valid[i]) continue;
-        const float* v = &acc[4 * j + 2 * i];
-        const float* g = &acc[4 * (j + BN / 16) + 2 * i];
-        // reference: x, gate = proj(x).chunk(2) are fp16 tensors; x * gelu(gate) in fp16 (attention.py:50-51)
-        const __half2 a = __floats2half2_rn(fmaf(v[0], alpha, h2lo(bv)), fmaf(v[1], alpha, h2hi(bv)));
-        const float2 gf = __half22float2(__floats2half2_rn(fmaf(g[0], alpha, h2lo(bg)), fmaf(g[1], alpha, h2hi(bg))));
-        put(i, c, __hmul2(a, __floats2half2_rn(gelu_sig(gf.x), gelu_sig(gf.y))));
+        put(i, c, geglu_pair(&acc[4 * j + 2 * i], &acc[4 * (j + BN / 16) + 2 * i], alpha, bv, bg));
       }
     }
     return;
@@ -292,17 +288,8 @@ __device__ __forceinline__ void gemm_stage_tile(const GemmParams& p, const float
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         if (!valid[i]) continue;
-        float v0 = fmaf(acc[4 * j + 2 * i], alpha, h2lo(bias[j]));
-        float v1 = fmaf(acc[4 * j + 2 * i + 1], alpha, h2hi(bias[j]));
-        if (rowadd_row[i]) {
-          // per-image row add (time embedding): (conv + bias) + emb -> act, the reference's order
-          v0 += h2lo(ra[i][jj]);
-          v1 += h2hi(ra[i][jj]);
-        }
-        if (act != PFD_ACT_NONE) {
-          v0 = act_apply(v0, act);
-          v1 = act_apply(v1, act);
-        }
+        float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+        epi_pair(v0, v1, alpha, bias[j], rowadd_row[i] != nullptr, ra[i][jj], act);
         put(i, 8 * j + cq, __floats2half2_rn(v0, v1));
       }
     }
@@ -453,22 +440,16 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const float (
       const int c = 8 * j + cq;               // value column inside the tile; its gate is column c + BN / 2
       const int col = col_base + c;
       if (col >= n_out) continue;
-      float bv0 = 0.f, bv1 = 0.f, bg0 = 0.f, bg1 = 0.f;
+      uint32_t bv = 0u, bg = 0u;
       if (p.bias) {
-        const uint32_t bv = ldg_h2(p.bias + (long long)n_tile * BN + c);
-        const uint32_t bg = ldg_h2(p.bias + (long long)n_tile * BN + BN / 2 + c);
-        bv0 = h2lo(bv); bv1 = h2hi(bv); bg0 = h2lo(bg); bg1 = h2hi(bg);
+        bv = ldg_h2(p.bias + (long long)n_tile * BN + c);
+        bg = ldg_h2(p.bias + (long long)n_tile * BN + BN / 2 + c);
       }
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         if (!valid[i]) continue;
-        const float* v = &acc[4 * j + 2 * i];
-        const float* g = &acc[4 * (j + BN / 16) + 2 * i];
-        // reference: x, gate = proj(x).chunk(2) are fp16 tensors; x * gelu(gate) in fp16 (attention.py:50-51)
-        const __half2 a = __floats2half2_rn(fmaf(v[0], alpha, bv0), fmaf(v[1], alpha, bv1));
-        const float2 gf = __half22float2(__floats2half2_rn(fmaf(g[0], alpha, bg0), fmaf(g[1], alpha, bg1)));
-        const __half2 o = __hmul2(a, __floats2half2_rn(gelu_sig(gf.x), gelu_sig(gf.y)));
-        const float2 of = __half22float2(o);
+        const float2 of = __half22float2(
+            geglu_pair(&acc[4 * j + 2 * i], &acc[4 * (j + BN / 16) + 2 * i], alpha, bv, bg));
         store2(i, col, of.x, of.y);
       }
     }
@@ -479,26 +460,13 @@ __device__ __forceinline__ void gemm_epilogue(const GemmParams& p, const float (
   for (int j = 0; j < BN / 8; ++j) {
     const int col = col_base + 8 * j + cq;
     if (col >= n_out) continue;
-    float b0 = 0.f, b1 = 0.f;
-    if (p.bias) {
-      const uint32_t b = ldg_h2(p.bias + col);
-      b0 = h2lo(b); b1 = h2hi(b);
-    }
+    const uint32_t b = p.bias ? ldg_h2(p.bias + col) : 0u;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       if (!valid[i]) continue;
-      float v0 = fmaf(acc[4 * j + 2 * i], alpha, b0);
-      float v1 = fmaf(acc[4 * j + 2 * i + 1], alpha, b1);
-      if (rowadd_row[i]) {
-        // per-image row add (time embedding): (conv + bias) + emb -> act, the reference's order
-        const uint32_t r = ldg_h2(rowadd_row[i] + col);
-        v0 += h2lo(r);
-        v1 += h2hi(r);
-      }
-      if (act != PFD_ACT_NONE) {
-        v0 = act_apply(v0, act);
-        v1 = act_apply(v1, act);
-      }
+      const uint32_t r = rowadd_row[i] ? ldg_h2(rowadd_row[i] + col) : 0u;
+      float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+      epi_pair(v0, v1, alpha, b, rowadd_row[i] != nullptr, r, act);
       store2(i, col, v0, v1);
     }
   }
@@ -661,14 +629,8 @@ splitk_finish_kernel(const __grid_constant__ GemmParams p) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
     const int v = (int)(i % vecs);
     const long long prow = i / vecs;
-    const int m_tile = (int)(prow / BM), row = (int)(prow % BM);
-    const int tx = m_tile % p.tiles_w;
-    const int ty = (m_tile / p.tiles_w) % p.tiles_h;
-    const int tn = m_tile / (p.tiles_w * p.tiles_h);
-    const int x = tx * p.bw + row % p.bw;
-    const int y = ty * p.bh + (row / p.bw) % p.bh;
-    const int n = tn * p.bn + row / (p.bw * p.bh);
-    if (x >= p.W || y >= p.H || n >= p.NB) continue;
+    const TileRow r = tile_row(p, tile_origin(p, (int)(prow / BM)), (int)(prow % BM));
+    if (!r.valid) continue;
     const int col = v * 8;
     float acc[8];
 #pragma unroll
@@ -679,25 +641,16 @@ splitk_finish_kernel(const __grid_constant__ GemmParams p) {
       acc[0] += a.x; acc[1] += a.y; acc[2] += a.z; acc[3] += a.w;
       acc[4] += b.x; acc[5] += b.y; acc[6] += b.z; acc[7] += b.w;
     }
-    float bv[8];
+    uint4 bv = make_uint4(0, 0, 0, 0), rv = bv;
+    if (p.bias) bv = __ldg(reinterpret_cast<const uint4*>(p.bias + col));
+    if (p.rowadd) rv = __ldg(reinterpret_cast<const uint4*>(p.rowadd + (long long)r.n * p.rowadd_ld + col));
+    const uint32_t* b2 = &bv.x;
+    const uint32_t* r2 = &rv.x;
 #pragma unroll
-    for (int k = 0; k < 8; ++k) bv[k] = 0.f;
-    if (p.bias) load8h(p.bias + col, bv);
-#pragma unroll
-    for (int k = 0; k < 8; ++k) acc[k] = fmaf(acc[k], p.alpha, bv[k]);
-    if (p.rowadd) {
-      float rv[8];
-      load8h(p.rowadd + (long long)n * p.rowadd_ld + col, rv);
-#pragma unroll
-      for (int k = 0; k < 8; ++k) acc[k] += rv[k];
-    }
-    if (p.act != PFD_ACT_NONE) {
-#pragma unroll
-      for (int k = 0; k < 8; ++k) acc[k] = act_apply(acc[k], p.act);
-    }
+    for (int k = 0; k < 4; ++k)
+      epi_pair(acc[2 * k], acc[2 * k + 1], p.alpha, b2[k], p.rowadd != nullptr, r2[k], p.act);
     // fp16(act(...)), then the residual added in fp16: the same rounding as the staged epilogue
-    const long long row_off = (long long)(n / p.ndiv) * p.so_n1 + (long long)(n % p.ndiv) * p.so_n0 +
-                              (long long)y * p.so_y + (long long)x * p.so_x;
+    const long long row_off = out_row_off(p, r);
     if (p.vec_ok) {
       const long long off = row_off + out_col_off(p, col);
       uint4 o;
@@ -705,8 +658,8 @@ splitk_finish_kernel(const __grid_constant__ GemmParams p) {
 #pragma unroll
       for (int k = 0; k < 4; ++k) oh[k] = __floats2half2_rn(acc[2 * k], acc[2 * k + 1]);
       if (p.residual) {
-        const uint4 r = __ldg(reinterpret_cast<const uint4*>(p.residual + off));
-        const __half2* rh = reinterpret_cast<const __half2*>(&r);
+        const uint4 res = __ldg(reinterpret_cast<const uint4*>(p.residual + off));
+        const __half2* rh = reinterpret_cast<const __half2*>(&res);
 #pragma unroll
         for (int k = 0; k < 4; ++k) oh[k] = __hadd2(oh[k], rh[k]);
       }
@@ -728,75 +681,6 @@ splitk_finish_kernel(const __grid_constant__ GemmParams p) {
 // Size of the split-K workspace, which also bounds the partials of a split-K plan.  It decides which shapes are split
 // and so the bits of their results: keep it at 64 MiB - 4 KiB.
 constexpr size_t SPLITK_WS_BYTES = (64ull << 20) - 4096;
-// One fp32 split-K workspace per DEVICE, allocated by the first pfd_gemm_f16 call on that device that is not
-// inside a stream capture (cudaMalloc is illegal while capturing) - i.e. in the eager warm-up pass that every
-// graph-captured path of this package runs first - and then shared by the eager and the captured launches, so
-// that graph replay and eager execution choose the same split configuration (r1 advisor finding: the old
-// per-stream map was always empty on torch's capture stream, silently disabling split-K in every replayed path).
-// Launches of one device are stream-ordered by the callers (one request at a time, SURVEY.md 8b), so one buffer
-// per device is enough.
-static float* splitk_workspace(cudaStream_t st) {
-  constexpr int MAX_DEV = 64;
-  static std::mutex mu;
-  static float* ws[MAX_DEV] = {nullptr};
-  int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= MAX_DEV) return nullptr;
-  std::lock_guard<std::mutex> lk(mu);
-  if (ws[dev]) return ws[dev];
-  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-  if (cudaStreamIsCapturing(st, &cs) != cudaSuccess || cs != cudaStreamCaptureStatusNone) {
-    (void)cudaGetLastError();
-    return nullptr;
-  }
-  float* pnew = nullptr;
-  if (cudaMalloc(&pnew, SPLITK_WS_BYTES) != cudaSuccess) {
-    (void)cudaGetLastError();
-    return nullptr;
-  }
-  ws[dev] = pnew;
-  return pnew;
-}
-
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
-                                  const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                  const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess) {
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-    }
-  }
-  return fn;
-}
-
-static int encode_map(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims,
-                      const cuuint64_t* strides_bytes, const cuuint32_t* box,
-                      const cuuint32_t* estr, const char* what,
-                      CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
-  EncodeTiledFn fn = get_encode_fn();
-  if (!fn) return set_error("cuTensorMapEncodeTiled entry point unavailable (no CUDA driver?)");
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank, const_cast<void*>(ptr), dims,
-                  strides_bytes, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    return set_error(
-        "tensor map (%s) encode failed: CUresult %d rank %d dims[%llu,%llu,%llu,%llu] "
-        "strides[%llu,%llu,%llu] box[%u,%u,%u,%u] ptr %p",
-        what, (int)r, rank, (unsigned long long)dims[0], (unsigned long long)dims[1],
-        (unsigned long long)(rank > 2 ? dims[2] : 0), (unsigned long long)(rank > 3 ? dims[3] : 0),
-        (unsigned long long)strides_bytes[0], (unsigned long long)(rank > 2 ? strides_bytes[1] : 0),
-        (unsigned long long)(rank > 3 ? strides_bytes[2] : 0), box[0], box[1], rank > 2 ? box[2] : 0,
-        rank > 3 ? box[3] : 0, ptr);
-  }
-  return 0;
-}
 
 static inline long long cdivll(long long a, long long b) { return (a + b - 1) / b; }
 
@@ -813,13 +697,7 @@ static int launch_gemm(const GemmParams& p, int grid, cudaStream_t stream) {
             "splits=%d grid=%d batched=%d vec=%d plain=%d\n", (long long)p.W * p.H * p.NB, p.N, p.num_kb * BK,
             p.nseg, p.taps[0], p.stride, p.act, p.bias != nullptr, p.residual != nullptr, p.rowadd != nullptr, BN,
             p.splits, grid, p.b_batched, p.vec_ok, (int)(p.cdiv >= p.N));
-  static bool attr_done = false;
-  if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_BYTES);
-    if (e != cudaSuccess) return set_error("cudaFuncSetAttribute(gemm BN=%d): %s", BN, cudaGetErrorString(e));
-    attr_done = true;
-  }
+  if (int rc = smem_opt_in<gemm_wgmma_kernel<BN>>(Cfg::SMEM_BYTES, "gemm_wgmma_kernel")) return rc;
   launch_k(gemm_wgmma_kernel<BN>, dim3(grid), dim3(GEMM_THREADS), Cfg::SMEM_BYTES, stream, p);
   return check_launch("pfd_gemm_f16");
 }
@@ -941,12 +819,12 @@ extern "C" PFD_API int pfd_gemm_f16(const pfd_gemm_desc* d) {
     cuuint64_t strides[3] = {(cuuint64_t)d->a_sx[s] * 2, (cuuint64_t)d->a_sy[s] * 2, (cuuint64_t)d->a_sn[s] * 2};
     cuuint32_t box[4] = {(cuuint32_t)BK, (cuuint32_t)(bw * d->stride), (cuuint32_t)(bh * d->stride), (cuuint32_t)bn};
     cuuint32_t estr[4] = {1, (cuuint32_t)d->stride, (cuuint32_t)d->stride, 1};
-    if (int rc = encode_map(&p.tmA[s], d->a_ptr[s], 4, dims, strides, box, estr, "A")) return rc;
+    if (int rc = encode_tensor_map_f16(&p.tmA[s], d->a_ptr[s], 4, dims, strides, box, estr, "A")) return rc;
   }
   p.num_kb = num_kb;
   p.kb_per_split = num_kb;
   cudaStream_t st = static_cast<cudaStream_t>(d->stream);
-  float* const skws = splitk_workspace(st);     // allocated by the first eager call on this device
+  float* const skws = static_cast<float*>(device_scratch(SCRATCH_SPLITK, SPLITK_WS_BYTES, 0, st));
   // ---- split-K for long-K problems that cannot fill the machine (8x8-level convs): fewer, wider N tiles
   //      (less A re-read through L2) x several K slices, fp32 partials reduced by splitk_finish_kernel.
   //      Never in deterministic mode: whether it fires depends on M and the SM count, and it regroups the K sum.
@@ -985,7 +863,7 @@ extern "C" PFD_API int pfd_gemm_f16(const pfd_gemm_desc* d) {
     cuuint64_t strides[2] = {(cuuint64_t)d->K * 2, (cuuint64_t)bs * 2};
     cuuint32_t box[3] = {(cuuint32_t)BK, (cuuint32_t)BNsel, 1};
     cuuint32_t estr[3] = {1, 1, 1};
-    if (int rc = encode_map(&p.tmB, d->b_ptr, 3, dims, strides, box, estr, "B")) return rc;
+    if (int rc = encode_tensor_map_f16(&p.tmB, d->b_ptr, 3, dims, strides, box, estr, "B")) return rc;
   }
   const long long total = m_tiles * p.n_tiles * p.splits;
   int grid = (int)(total < sms ? total : sms);

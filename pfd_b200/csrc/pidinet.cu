@@ -401,12 +401,7 @@ extern "C" PFD_API int pfd_pidinet_cdcm_f16(const void* m, int32_t B, int32_t h,
     return set_error("pfd_pidinet_cdcm_f16: bad arguments (B=%d h=%d w=%d)", B, h, w);
   if (misaligned(m) || misaligned(wpk) || misaligned(u))
     return set_error("pfd_pidinet_cdcm_f16: m, wpk and u must be 16-byte aligned");
-  static bool attr_done = false;
-  if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(pidinet_cdcm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CD_SMEM);
-    if (e != cudaSuccess) return set_error("cudaFuncSetAttribute(pidinet_cdcm): %s", cudaGetErrorString(e));
-    attr_done = true;
-  }
+  if (int rc = smem_opt_in<pidinet_cdcm_kernel>((int)CD_SMEM, "pidinet_cdcm_kernel")) return rc;
   const dim3 grid((w + CD_T - 1) / CD_T, (h + CD_T - 1) / CD_T, B);
   launch_k(pidinet_cdcm_kernel, grid, dim3(CD_THREADS), CD_SMEM, static_cast<cudaStream_t>(stream),
            static_cast<const __half*>(m), (int)h, (int)w, static_cast<const uint2*>(wpk), u);
