@@ -181,9 +181,8 @@ class AutoencoderKL(nn.Module):
         B = x.shape[0]
         nv.gn_reset()
         h = nv.nchw_to_nhwc(x, mul=2.0, add=-1.0)                          # [B,H,W,3]
-        w, b, kpad = pk_conv3_small(enc.conv_in)
-        _, H, W, _ = h.shape
-        h = nv.linear(nv.im2col3x3(h, kpad).reshape(B * H * W, kpad), w, b).reshape(B, H, W, w.shape[0])
+        w, b = pk_conv3_small(enc.conv_in)
+        h = nv.conv3x3_im2col(h, w, b)
         for lvl in range(enc.num_resolutions):
             for rb in enc.down[lvl].block:
                 h = run_vae_resnet(rb, h)
@@ -215,9 +214,8 @@ class AutoencoderKL(nn.Module):
         zc = nv.nchw_to_nhwc(z if z.dtype == torch.float32 else z.to(torch.float16), cpad=8)
         wq, bq = pk_lin(self.post_quant_conv)                              # [8, 8] zero-padded 4x4
         h = nv.linear(zc.reshape(B * H * W, 8), wq, bq, alpha=pre_scale).reshape(B, H, W, 8)
-        w, b, kpad = cached_conv_in(dec.conv_in, Cz)
-        col = nv.im2col3x3(h, kpad)
-        h = nv.linear(col.reshape(B * H * W, kpad), w, b).reshape(B, H, W, w.shape[0])
+        w, b = cached_conv_in(dec.conv_in, Cz)
+        h = nv.conv3x3_im2col(h, w, b)
         h = run_vae_resnet(dec.mid.block_1, h)
         h = run_vae_attn(dec.mid.attn_1, h)
         h = run_vae_resnet(dec.mid.block_2, h)
@@ -264,5 +262,5 @@ def cached_conv_in(conv: Conv2d, cz: int):
         o = conv.weight.shape[0]
         w = torch.zeros((o, 3, 3, 8), device=conv.weight.device, dtype=torch.float16)
         w[..., :cz] = fp16(conv.weight).permute(0, 2, 3, 1)
-        return w.reshape(o, 72).contiguous(), fp16(conv.bias), 72
+        return w.reshape(o, 72).contiguous(), fp16(conv.bias)
     return cached(conv, "conv_in8", [conv.weight, conv.bias], build)

@@ -107,15 +107,13 @@ class ControlNet(nn.Module):
         for i, conv in enumerate(convs):
             act = nv.ACT_SILU if i < len(convs) - 1 else nv.ACT_NONE
             s = conv.stride[0]
-            B, H, W, C = h.shape
+            C = h.shape[3]
             if C % 8 == 0 and C >= 16:
                 w, b = pk_conv3(conv)
                 h = nv.conv3x3(h, w, b, stride=s, act=act)
             else:
-                w, b, kpad = pk_conv3_small(conv)
-                col = nv.im2col3x3(h, kpad, stride=s)
-                Ho, Wo = col.shape[1], col.shape[2]
-                h = nv.linear(col.reshape(B * Ho * Wo, kpad), w, b, act=act).reshape(B, Ho, Wo, w.shape[0])
+                w, b = pk_conv3_small(conv)
+                h = nv.conv3x3_im2col(h, w, b, stride=s, act=act)
         return h
 
     def forward(self, x, hint, timesteps, context, kv=None, hint_feat=None, **kwargs) -> List[torch.Tensor]:
@@ -142,10 +140,8 @@ class ControlNet(nn.Module):
                     w, b = pk_conv3(layer.op)
                     h = nv.conv3x3(h, w, b, stride=2)
                 elif isinstance(layer, Conv2d):
-                    w, b, kpad = pk_conv3_small(layer)
-                    B, H, W, _ = h.shape
-                    col = nv.im2col3x3(h, kpad)
-                    h = nv.linear(col.reshape(B * H * W, kpad), w, b).reshape(B, H, W, w.shape[0])
+                    w, b = pk_conv3_small(layer)
+                    h = nv.conv3x3_im2col(h, w, b)
             if guided is not None:
                 B = h.shape[0]
                 if guided.shape[0] == B:

@@ -94,10 +94,7 @@ class ControlNetHED(nn.Module):
         for bi, (layer, (pw, pb)) in enumerate(zip(convs, projs)):
             for ci, (w, b) in enumerate(layer):
                 if bi == 0 and ci == 0:
-                    kpad = w.shape[1]
-                    Bh, Hh, Wh, _ = h.shape
-                    col = nv.im2col3x3(h, kpad)
-                    h = nv.linear(col.reshape(Bh * Hh * Wh, kpad), w, b, act=nv.ACT_RELU).reshape(Bh, Hh, Wh, w.shape[0])
+                    h = nv.conv3x3_im2col(h, w, b, act=nv.ACT_RELU)
                 else:
                     h = nv.conv3x3(h, w, b, act=nv.ACT_RELU)
             side, pooled = nv.hed_pool_side(h, pw, pb, pool=bi < len(convs) - 1)

@@ -130,14 +130,14 @@ def pk_conv3(conv: nn.Conv2d, skip: Optional[nn.Conv2d] = None) -> Tuple[torch.T
     return cached(conv, "conv3" + ("+skip" if skip is not None else ""), params, build)
 
 
-def pk_conv3_small(conv: nn.Conv2d) -> Tuple[torch.Tensor, Optional[torch.Tensor], int]:
-    """3x3 conv with tiny Cin (im2col path): weights [O, Kpad], Kpad = ceil8(9*Cin)."""
+def pk_conv3_small(conv: nn.Conv2d) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+    """3x3 conv with tiny Cin (im2col path, native.conv3x3_im2col): weights [O, Kpad], Kpad = ceil8(9*Cin)."""
     def build():
         w = pad_cols(pack_conv(conv.weight))
         b = fp16(conv.bias)
         if w.shape[0] % 8:
             w, b = pad_rows(w), (pad_rows(b) if b is not None else None)
-        return w, b, w.shape[1]
+        return w, b
     return cached(conv, "conv3s", [conv.weight, conv.bias], build)
 
 

@@ -3,42 +3,28 @@
 This is the *only* way compute reaches the GPU in this package: there is no torch / CPU fallback.
 If the shared library is missing or a call fails, a ``RuntimeError`` is raised.
 
-Tensors are torch CUDA fp16 tensors used purely as device-memory handles (``data_ptr()``); the
-stream is torch's current stream so calls can be captured into CUDA graphs.
+The argument and return types of every entry point come from its prototype in ``include/pfd_b200.h``.  Tensors go
+into pointer arguments as they are (``DevicePtr``); the stream is torch's current stream so calls can be captured
+into CUDA graphs.
 """
 from __future__ import annotations
 
 import ctypes
 import os
+import re
 from ctypes import POINTER, c_char_p, c_float, c_int32, c_int64, c_uint32, c_void_p
-from typing import Optional, Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 # PFD_B200_LIB: load another build of the same ABI (A/B runs of compile-time variants); default = the in-tree library
 LIB_PATH = os.environ.get("PFD_B200_LIB") or os.path.join(_HERE, "libpfd_b200.so")
+HEADER = os.path.join(_HERE, os.pardir, "include", "pfd_b200.h")
 
+# mirrors of the header's #defines (tests/test_abi_cpu.py keeps them equal)
 PFD_MAX_SEG = 3
 ACT_NONE, ACT_SILU, ACT_GELU, ACT_RELU, ACT_GEGLU = 0, 1, 2, 3, 4
-
-EXPORTS = [
-    "pfd_version", "pfd_last_error", "pfd_launch_count", "pfd_set_option", "pfd_gemm_f16", "pfd_groupnorm_f16",
-    "pfd_layernorm_f16", "pfd_softmax_f16", "pfd_timestep_embedding_f16", "pfd_upsample2x_f16",
-    "pfd_nchw_to_nhwc_f16", "pfd_nhwc_to_nchw_f16", "pfd_im2col3x3_f16", "pfd_axpby_f16",
-    "pfd_add_rowvec_f16", "pfd_ddim_step_f16", "pfd_window_gather_f16", "pfd_window_scatter_f16",
-    "pfd_patch_merge_gather_f16", "pfd_patchify_f16", "pfd_flash_attn_f16",
-    "pfd_flash_attn_strided_f16", "pfd_ddim_begin_step", "pfd_vae_posterior_f16",
-    "pfd_canny_workspace_bytes", "pfd_canny_f32", "pfd_image_u8_roundtrip_f32",
-    "pfd_hed_input_f16", "pfd_hed_pool_side_f16", "pfd_hed_fuse_f32",
-    "pfd_timestep_embedding_ft_f16", "pfd_ksampler_step_f32", "pfd_ksampler_begin_step", "pfd_randn_f16",
-    "pfd_scribble_hed_f32", "pfd_scribble_blur_u8", "pfd_scribble_xdog_f32",
-    "pfd_pidinet_dw_f16", "pfd_pidinet_reduce_f16", "pfd_pidinet_cdcm_f16", "pfd_pidinet_side_f32",
-    "pfd_pidinet_fuse_f32", "pfd_mlsd_input_f16", "pfd_mlsd_dw_f16", "pfd_mlsd_upsample_f16", "pfd_mlsd_head_f32",
-    "pfd_mlsd_decode_f32", "pfd_mlsd_draw_f32", "pfd_openpose_input_f16", "pfd_openpose_pool_f16", "pfd_im2col7x7_f16",
-    "pfd_openpose_head_f32", "pfd_openpose_resize_f32", "pfd_openpose_peaks_f32", "pfd_openpose_assemble_f32",
-    "pfd_openpose_draw_f32",
-]
 PFD_KSAMPLER_NCOEF = 6
 PFD_HED_MAX_SIDES = 5
 PFD_PIDINET_SIDE_PARAMS = 161
@@ -80,11 +66,65 @@ class GemmDesc(ctypes.Structure):
     ]
 
 
+class DevicePtr(c_void_p):
+    """Type of every pointer argument: a CUDA tensor passes its data_ptr(), None passes NULL, and whatever c_void_p
+    accepts (ints, ctypes arrays, byref) passes unchanged.  A tensor that is not on a CUDA device is refused before
+    the call (ctypes.ArgumentError naming the argument's position) instead of reaching a kernel as a host address."""
+
+    @classmethod
+    def from_param(cls, obj):
+        if isinstance(obj, torch.Tensor):
+            if not obj.is_cuda:
+                raise TypeError(f"expected a CUDA tensor, got a {obj.dtype} tensor on {obj.device}")
+            obj = obj.data_ptr()
+        return c_void_p.from_param(obj)
+
+
+# C type of the header -> ctypes type; any other pointer type is a DevicePtr
+_CTYPES = {"int": c_int32, "int32_t": c_int32, "uint32_t": c_uint32, "int64_t": c_int64, "float": c_float,
+           "const char*": c_char_p, "const pfd_gemm_desc*": POINTER(GemmDesc)}
+
+
+def _prototypes() -> Dict[str, Tuple[str, List[str]]]:
+    """{name: (return type, [parameter types])} of every PFD_API prototype in HEADER, types with normalised spaces."""
+    with open(HEADER) as f:
+        src = re.sub(r"/\*.*?\*/|//[^\n]*", "", f.read(), flags=re.S)
+    norm = lambda t: re.sub(r"\s*\*", "*", " ".join(t.split()))
+    protos = {}
+    for ret, name, params in re.findall(r"PFD_API\s+([\w\s\*]+?)\s*\b(pfd_\w+)\s*\(([^)]*)\)", src):
+        params = [] if params.strip() == "void" else [re.sub(r"\w+\s*$", "", p) for p in params.split(",")]
+        protos[name] = (norm(ret), [norm(p) for p in params])
+    return protos
+
+
+def _ctype(name: str, t: str):
+    if t in _CTYPES:
+        return _CTYPES[t]
+    if t.endswith("*"):
+        return DevicePtr
+    raise RuntimeError(f"{name}: the C type '{t}' of include/pfd_b200.h has no ctypes mapping in native._CTYPES")
+
+
+EXPORTS = tuple(_prototypes())
 _lib = None
 
 
+def _declare(lib):
+    """Set argtypes and restype of every function the header declares on lib; raises on a type without a mapping and
+    on declared functions lib lacks."""
+    protos = _prototypes()
+    missing = [name for name in protos if not hasattr(lib, name)]
+    if missing:
+        raise RuntimeError(f"{LIB_PATH} lacks functions that include/pfd_b200.h declares: {', '.join(missing)}")
+    for name, (ret, params) in protos.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = _ctype(name, ret), [_ctype(name, t) for t in params]
+    return lib
+
+
 def load() -> ctypes.CDLL:
-    """Load the shared library (once). Raises if it has not been built (``__graft_entry__.build``)."""
+    """Load the shared library (once) and declare its functions from the header.  Raises if it has not been built
+    (``__graft_entry__.build``)."""
     global _lib
     if _lib is not None:
         return _lib
@@ -92,102 +132,8 @@ def load() -> ctypes.CDLL:
         raise RuntimeError(
             f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
             "(there is no CPU/PyTorch fallback for the pfd_b200 kernels)")
-    lib = ctypes.CDLL(LIB_PATH)
-    lib.pfd_version.restype = c_int32
-    lib.pfd_last_error.restype = c_char_p
-    lib.pfd_launch_count.restype = c_int64
-    lib.pfd_set_option.argtypes = [c_char_p, c_int32]
-    lib.pfd_gemm_f16.argtypes = [POINTER(GemmDesc)]
-    lib.pfd_groupnorm_f16.argtypes = [c_void_p, c_int32, c_void_p, c_int32, c_int32, c_int64, c_int32,
-                                      c_void_p, c_void_p, c_float, c_int32, c_void_p, c_void_p, c_int32, c_void_p]
-    lib.pfd_layernorm_f16.argtypes = [c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_float,
-                                      c_void_p, c_void_p]
-    lib.pfd_softmax_f16.argtypes = [c_void_p, c_int64, c_int32, c_int32, c_int64, c_float, c_void_p,
-                                    c_int32, c_void_p, c_int32, c_void_p]
-    lib.pfd_timestep_embedding_f16.argtypes = [c_void_p, c_int32, c_int32, c_float, c_void_p, c_void_p]
-    lib.pfd_timestep_embedding_ft_f16.argtypes = [c_void_p, c_int32, c_int32, c_float, c_void_p, c_void_p]
-    lib.pfd_upsample2x_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]
-    lib.pfd_nchw_to_nhwc_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
-                                         c_float, c_float, c_void_p, c_void_p]
-    lib.pfd_vae_posterior_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_float,
-                                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]
-    lib.pfd_nhwc_to_nchw_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_float,
-                                         c_float, c_float, c_float, c_void_p, c_void_p]
-    lib.pfd_im2col3x3_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
-                                      c_void_p, c_void_p]
-    lib.pfd_axpby_f16.argtypes = [c_void_p, c_float, c_void_p, c_float, c_int64, c_void_p, c_void_p]
-    lib.pfd_add_rowvec_f16.argtypes = [c_void_p, c_void_p, c_int64, c_int32, c_void_p, c_void_p]
-    lib.pfd_ddim_step_f16.argtypes = [c_void_p, c_void_p, c_int64, c_float, c_void_p, c_void_p, c_void_p,
-                                      c_void_p, c_void_p, c_float, c_void_p, c_void_p, c_void_p, c_void_p]
-    lib.pfd_window_gather_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
-                                          c_void_p, c_void_p]
-    lib.pfd_window_scatter_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
-                                           c_void_p, c_void_p, c_void_p]
-    lib.pfd_patch_merge_gather_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p,
-                                               c_void_p]
-    lib.pfd_patchify_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32,
-                                     c_void_p, c_void_p]
-    if True:
-        lib.pfd_flash_attn_f16.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32,
-                                           c_int32, c_int32, c_int32, c_int32, c_int32, c_float,
-                                           c_int64, c_int64, c_int64, c_int32, c_void_p]
-    lib.pfd_flash_attn_strided_f16.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32,
-                                               c_int32, c_int32, POINTER(c_int64), POINTER(c_int64),
-                                               POINTER(c_int64), c_float, c_int64, c_int64, c_void_p]
-    lib.pfd_ddim_begin_step.argtypes = [c_void_p, c_void_p, c_void_p, c_int32, c_void_p]
-    lib.pfd_ksampler_step_f32.argtypes = [c_void_p, c_int32, c_float, c_int64, c_void_p, c_void_p, c_int32, c_void_p,
-                                          c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
-                                          c_void_p]
-    lib.pfd_ksampler_begin_step.argtypes = [c_void_p, c_void_p, c_int32, c_void_p, c_int32, c_void_p]
-    lib.pfd_randn_f16.argtypes = [c_void_p, c_int32, c_int64, c_void_p, c_uint32, c_int32, c_void_p, c_float, c_void_p]
-    lib.pfd_canny_workspace_bytes.argtypes = [c_int32, c_int32, c_int32]
-    lib.pfd_canny_workspace_bytes.restype = c_int64
-    lib.pfd_canny_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p,
-                                  POINTER(c_int32), c_void_p]
-    lib.pfd_image_u8_roundtrip_f32.argtypes = [c_void_p, c_int32, c_int64, c_void_p, c_void_p]
-    lib.pfd_hed_input_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_float,
-                                      c_void_p, c_void_p]
-    lib.pfd_hed_pool_side_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p,
-                                          c_void_p, c_void_p]
-    lib.pfd_hed_fuse_f32.argtypes = [POINTER(c_void_p), POINTER(c_int32), POINTER(c_int32), c_int32, c_int32, c_int32,
-                                     c_int32, c_float, c_void_p, c_void_p]
-    lib.pfd_scribble_hed_f32.argtypes = [c_void_p, c_int64, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]
-    lib.pfd_scribble_blur_u8.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]
-    lib.pfd_scribble_xdog_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]
-    lib.pfd_pidinet_dw_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p,
-                                       c_void_p, c_void_p, c_void_p]
-    lib.pfd_pidinet_reduce_f16.argtypes = [c_void_p, c_int64, c_int32, c_void_p, c_void_p, c_void_p, c_void_p]
-    lib.pfd_pidinet_cdcm_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]
-    lib.pfd_pidinet_side_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p]
-    lib.pfd_pidinet_fuse_f32.argtypes = [POINTER(c_void_p), POINTER(c_int32), POINTER(c_int32), c_int32, c_int32,
-                                         c_int32, c_void_p, c_void_p, c_void_p]
-    lib.pfd_mlsd_input_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]
-    lib.pfd_mlsd_dw_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p,
-                                    c_void_p]
-    lib.pfd_mlsd_upsample_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_int64, c_void_p]
-    lib.pfd_mlsd_head_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_void_p,
-                                      c_void_p]
-    lib.pfd_mlsd_decode_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_float, c_float, c_void_p, c_void_p,
-                                        c_void_p, c_void_p]
-    lib.pfd_mlsd_draw_f32.argtypes = [c_void_p, c_void_p, c_int32, c_int32, c_int32, c_void_p, c_void_p]
-    lib.pfd_openpose_input_f16.argtypes = [c_void_p] + [c_int32] * 11 + [c_void_p, c_void_p, c_int32] * 2 + \
-        [c_void_p, c_void_p]
-    lib.pfd_openpose_pool_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]
-    lib.pfd_im2col7x7_f16.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p]
-    lib.pfd_openpose_head_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_void_p, c_int32,
-                                          c_int32, c_void_p, c_int32, c_int32, c_void_p]
-    lib.pfd_openpose_resize_f32.argtypes = [c_void_p] + [c_int32] * 11 + [c_void_p, c_void_p, c_int32] * 2 + \
-        [c_void_p, c_void_p]
-    lib.pfd_openpose_peaks_f32.argtypes = [c_void_p, c_int32, c_int32, c_int32] + [c_void_p] * 8
-    lib.pfd_openpose_assemble_f32.argtypes = [c_void_p] + [c_int32] * 9 + [c_void_p, c_void_p, c_int32] * 2 + \
-        [c_void_p] * 9
-    lib.pfd_openpose_draw_f32.argtypes = [c_void_p, c_void_p, c_void_p, c_int32, c_int32, c_int32] + [c_void_p] * 5
-    for name in EXPORTS:
-        if hasattr(lib, name) and name not in ("pfd_version", "pfd_last_error", "pfd_launch_count",
-                                               "pfd_canny_workspace_bytes"):
-            getattr(lib, name).restype = c_int32
-    _lib = lib
-    return lib
+    _lib = _declare(ctypes.CDLL(LIB_PATH))
+    return _lib
 
 
 def _check(rc: int, what: str) -> None:
@@ -242,9 +188,16 @@ def launch_count() -> int:
 
 
 def _p(t: Optional[torch.Tensor]) -> Optional[int]:
+    """Address of an optional tensor, for the pointer fields of GemmDesc (function arguments take tensors directly)."""
     if t is None:
         return None
     return t.data_ptr()
+
+
+def _call(name: str, *args) -> None:
+    """The library function `name` on (*args, current stream); raises RuntimeError with the library's error text when
+    it fails.  The library is looked up on every call, so a test can replace load()."""
+    _check(getattr(load(), name)(*args, stream_ptr()), name)
 
 
 def _chk16(t: torch.Tensor, name: str) -> None:
@@ -453,9 +406,7 @@ def groupnorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: flo
             raise RuntimeError("groupnorm: batch too large for the statistics scratch")
         ws_ptr, zero = ring["buf"].data_ptr() + _GN_SLOTS * _GN_SLOT_BYTES, 1    # shared fallback slot, zeroed per call
         ring["next"] = _GN_SLOTS
-    _check(load().pfd_groupnorm_f16(x.data_ptr(), C1, _p(x2), C2, NB, H * W, groups, gamma.data_ptr(),
-                                    beta.data_ptr(), eps, int(silu), out.data_ptr(), ws_ptr, zero, stream_ptr()),
-           "pfd_groupnorm_f16")
+    _call("pfd_groupnorm_f16", x, C1, x2, C2, NB, H * W, groups, gamma, beta, eps, int(silu), out, ws_ptr, zero)
     return out
 
 
@@ -465,8 +416,7 @@ def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: flo
     rows = x.numel() // C
     if out is None:
         out = torch.empty_like(x)
-    _check(load().pfd_layernorm_f16(x.data_ptr(), _p(residual), rows, C, gamma.data_ptr(), beta.data_ptr(),
-                                    eps, out.data_ptr(), stream_ptr()), "pfd_layernorm_f16")
+    _call("pfd_layernorm_f16", x, residual, rows, C, gamma, beta, eps, out)
     return out
 
 
@@ -488,8 +438,7 @@ def softmax_(s: torch.Tensor, scale: float, *, bias: Optional[torch.Tensor] = No
             if tuple(t.shape) != (max(n, 1), rows, cols) or not t.is_contiguous():
                 raise ValueError(f"softmax_: {name} must be a contiguous [{max(n, 1)}, {rows}, {cols}] tensor, "
                                  f"got {tuple(t.shape)} with strides {t.stride()}")
-    _check(load().pfd_softmax_f16(s.data_ptr(), batch, rows, cols, s.stride(1), scale, _p(bias), nheads,
-                                  _p(mask), nwin, stream_ptr()), "pfd_softmax_f16")
+    _call("pfd_softmax_f16", s, batch, rows, cols, s.stride(1), scale, bias, nheads, mask, nwin)
     return s
 
 
@@ -497,11 +446,9 @@ def timestep_embedding(t: torch.Tensor, dim: int, max_period: float = 10000.0) -
     """[cos | sin] embedding of int64 timesteps (the DDIM sampler) or float32 fractional ones (the k-samplers)."""
     out = torch.empty((t.shape[0], dim), device=t.device, dtype=torch.float16)
     if t.dtype == torch.int64:
-        _check(load().pfd_timestep_embedding_f16(t.data_ptr(), t.shape[0], dim, max_period, out.data_ptr(),
-                                                 stream_ptr()), "pfd_timestep_embedding_f16")
+        _call("pfd_timestep_embedding_f16", t, t.shape[0], dim, max_period, out)
     elif t.dtype == torch.float32:
-        _check(load().pfd_timestep_embedding_ft_f16(t.contiguous().data_ptr(), t.shape[0], dim, max_period,
-                                                    out.data_ptr(), stream_ptr()), "pfd_timestep_embedding_ft_f16")
+        _call("pfd_timestep_embedding_ft_f16", t.contiguous(), t.shape[0], dim, max_period, out)
     else:
         raise RuntimeError(f"timestep_embedding: int64 or float32 timesteps expected, got {t.dtype}")
     return out
@@ -511,8 +458,7 @@ def upsample2x(x: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Ten
     NB, H, W, C = x.shape
     if out is None:
         out = torch.empty((NB, 2 * H, 2 * W, C), device=x.device, dtype=torch.float16)
-    _check(load().pfd_upsample2x_f16(x.data_ptr(), NB, H, W, C, out.data_ptr(), stream_ptr()),
-           "pfd_upsample2x_f16")
+    _call("pfd_upsample2x_f16", x, NB, H, W, C, out)
     return out
 
 
@@ -525,8 +471,7 @@ def nchw_to_nhwc(x: torch.Tensor, cpad: Optional[int] = None, out: Optional[torc
         out = torch.empty((NB, H, W, cpad), device=x.device, dtype=torch.float16)
     if x.dtype not in (torch.float16, torch.float32):
         raise RuntimeError(f"nchw_to_nhwc: unsupported dtype {x.dtype}")
-    _check(load().pfd_nchw_to_nhwc_f16(x.data_ptr(), int(x.dtype == torch.float32), NB, C, H, W, cpad, mul, add,
-                                       out.data_ptr(), stream_ptr()), "pfd_nchw_to_nhwc_f16")
+    _call("pfd_nchw_to_nhwc_f16", x, int(x.dtype == torch.float32), NB, C, H, W, cpad, mul, add, out)
     return out
 
 
@@ -536,8 +481,7 @@ def nhwc_to_nchw(x: torch.Tensor, C: Optional[int] = None, *, mul: float = 1.0, 
     C = C or Cpad
     if out is None:
         out = torch.empty((NB, C, H, W), device=x.device, dtype=torch.float16)
-    _check(load().pfd_nhwc_to_nchw_f16(x.data_ptr(), NB, C, H, W, Cpad, mul, add, lo, hi, out.data_ptr(),
-                                       stream_ptr()), "pfd_nhwc_to_nchw_f16")
+    _call("pfd_nhwc_to_nchw_f16", x, NB, C, H, W, Cpad, mul, add, lo, hi, out)
     return out
 
 
@@ -546,17 +490,25 @@ def im2col3x3(x: torch.Tensor, kpad: int, stride: int = 1, out: Optional[torch.T
     Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
     if out is None:
         out = torch.empty((NB, Ho, Wo, kpad), device=x.device, dtype=torch.float16)
-    _check(load().pfd_im2col3x3_f16(x.data_ptr(), NB, H, W, C, stride, kpad, out.data_ptr(), stream_ptr()),
-           "pfd_im2col3x3_f16")
+    _call("pfd_im2col3x3_f16", x, NB, H, W, C, stride, kpad, out)
     return out
+
+
+def conv3x3_im2col(x: torch.Tensor, w: torch.Tensor, b: Optional[torch.Tensor] = None, *, stride: int = 1,
+                   act: int = ACT_NONE) -> torch.Tensor:
+    """3x3 / pad 1 convolution of channel-last x [NB, H, W, C] whose C is too small for conv3x3's TMA path (UNet / VAE
+    conv_in, the ControlNet hint stem, the annotators' RGB input): im2col3x3 to K = w.shape[1] columns, then linear.
+    w: [N, K] packed as k = tap*C + c, zero columns up to K -> [NB, Ho, Wo, N]."""
+    col = im2col3x3(x, w.shape[1], stride)
+    NB, Ho, Wo, K = col.shape
+    return linear(col.reshape(NB * Ho * Wo, K), w, b, act=act).reshape(NB, Ho, Wo, w.shape[0])
 
 
 def axpby(a: torch.Tensor, sa: float, b: Optional[torch.Tensor] = None, sb: float = 0.0,
           out: Optional[torch.Tensor] = None) -> torch.Tensor:
     if out is None:
         out = torch.empty_like(a)
-    _check(load().pfd_axpby_f16(a.data_ptr(), sa, _p(b), sb, a.numel(), out.data_ptr(), stream_ptr()),
-           "pfd_axpby_f16")
+    _call("pfd_axpby_f16", a, sa, b, sb, a.numel(), out)
     return out
 
 
@@ -564,8 +516,7 @@ def add_rowvec(a: torch.Tensor, row: torch.Tensor, out: Optional[torch.Tensor] =
     C = a.shape[-1]
     if out is None:
         out = torch.empty_like(a)
-    _check(load().pfd_add_rowvec_f16(a.data_ptr(), row.data_ptr(), a.numel() // C, C, out.data_ptr(),
-                                     stream_ptr()), "pfd_add_rowvec_f16")
+    _call("pfd_add_rowvec_f16", a, row, a.numel() // C, C, out)
     return out
 
 
@@ -575,18 +526,15 @@ def ddim_step(eps: torch.Tensor, x: torch.Tensor, guidance: float, coef: torch.T
               log_tab: Optional[torch.Tensor] = None, log_xt: Optional[torch.Tensor] = None,
               log_x0: Optional[torch.Tensor] = None) -> None:
     """Fused CFG combine + DDIM update (see pfd_ddim_step_f16); eps holds [uncond | cond] halves."""
-    _check(load().pfd_ddim_step_f16(eps.data_ptr(), x.data_ptr(), x.numel(), guidance, coef.data_ptr(),
-                                    _p(step), x_prev.data_ptr(), _p(pred_x0), _p(noise), float(temperature),
-                                    _p(log_tab), _p(log_xt), _p(log_x0), stream_ptr()),
-           "pfd_ddim_step_f16")
+    _call("pfd_ddim_step_f16", eps, x, x.numel(), guidance, coef, step, x_prev, pred_x0, noise, float(temperature),
+          log_tab, log_xt, log_x0)
 
 
 def ddim_begin_step(step: torch.Tensor, ttab: torch.Tensor, t_out: torch.Tensor) -> None:
     """Device-side loop header: step -= 1; t_out[:] = ttab[step] (see pfd_ddim_begin_step)."""
     if step.dtype != torch.int32 or ttab.dtype != torch.int64 or t_out.dtype != torch.int64:
         raise RuntimeError("ddim_begin_step: step int32, ttab / t_out int64 expected")
-    _check(load().pfd_ddim_begin_step(step.data_ptr(), ttab.data_ptr(), t_out.data_ptr(), t_out.numel(),
-                                      stream_ptr()), "pfd_ddim_begin_step")
+    _call("pfd_ddim_begin_step", step, ttab, t_out, t_out.numel())
 
 
 def ksampler_step(eps: torch.Tensor, cfg: bool, guidance: float, coef: torch.Tensor, step: torch.Tensor,
@@ -609,18 +557,15 @@ def ksampler_step(eps: torch.Tensor, cfg: bool, guidance: float, coef: torch.Ten
     _chk16(out, "ksampler_step out")
     if noise is not None:
         _chk16(noise, "ksampler_step noise")
-    _check(load().pfd_ksampler_step_f32(eps.data_ptr(), int(cfg), float(guidance), half_n, coef.data_ptr(),
-                                        step.data_ptr(), int(last_step), x.data_ptr(), d_prev.data_ptr(), _p(noise),
-                                        unet_in.data_ptr(), out.data_ptr(), _p(log_tab), _p(log_xt), _p(log_x0),
-                                        stream_ptr()), "pfd_ksampler_step_f32")
+    _call("pfd_ksampler_step_f32", eps, int(cfg), float(guidance), half_n, coef, step, int(last_step), x, d_prev, noise,
+          unet_in, out, log_tab, log_xt, log_x0)
 
 
 def ksampler_begin_step(step: torch.Tensor, ttab: torch.Tensor, t_out: torch.Tensor) -> None:
     """Device-side loop header: step += 1; t_out[:] = ttab[step] (see pfd_ksampler_begin_step)."""
     if step.dtype != torch.int32 or ttab.dtype != torch.float32 or t_out.dtype != torch.float32:
         raise RuntimeError("ksampler_begin_step: step int32, ttab / t_out float32 expected")
-    _check(load().pfd_ksampler_begin_step(step.data_ptr(), ttab.data_ptr(), ttab.numel(), t_out.data_ptr(),
-                                          t_out.numel(), stream_ptr()), "pfd_ksampler_begin_step")
+    _call("pfd_ksampler_begin_step", step, ttab, ttab.numel(), t_out, t_out.numel())
 
 
 def randn_f16(out: torch.Tensor, seeds: torch.Tensor, stream_id: int, draw: int = 0,
@@ -635,8 +580,8 @@ def randn_f16(out: torch.Tensor, seeds: torch.Tensor, stream_id: int, draw: int 
         raise RuntimeError(f"randn_f16: seeds must be a contiguous CUDA int64 tensor of {B} entries")
     if draw_dev is not None and (draw_dev.dtype != torch.int32 or not draw_dev.is_cuda):
         raise RuntimeError("randn_f16: draw_dev must be a CUDA int32 tensor")
-    _check(load().pfd_randn_f16(out.data_ptr(), B, out.numel() // B, seeds.data_ptr(), int(stream_id) & 0xffffffff,
-                                int(draw), _p(draw_dev), float(scale), stream_ptr()), "pfd_randn_f16")
+    _call("pfd_randn_f16", out, B, out.numel() // B, seeds, int(stream_id) & 0xffffffff, int(draw), draw_dev,
+          float(scale))
     return out
 
 
@@ -647,9 +592,8 @@ def vae_posterior(moments: torch.Tensor, zc: int, *, noise: Optional[torch.Tenso
     outs = {k: torch.empty((B, zc, H, W), device=moments.device, dtype=torch.float16) for k in want}
     if noise is not None and (noise.dtype != torch.float32 or not noise.is_contiguous()):
         noise = noise.to(torch.float32).contiguous()
-    _check(load().pfd_vae_posterior_f16(moments.data_ptr(), B, zc, H, W, cpad, _p(noise), scale,
-                                        _p(outs.get("mean")), _p(outs.get("logvar")), _p(outs.get("std")),
-                                        _p(outs.get("sample")), stream_ptr()), "pfd_vae_posterior_f16")
+    _call("pfd_vae_posterior_f16", moments, B, zc, H, W, cpad, noise, scale, outs.get("mean"), outs.get("logvar"),
+          outs.get("std"), outs.get("sample"))
     return outs
 
 
@@ -661,8 +605,7 @@ def canny(x: torch.Tensor, low: int = 100, high: int = 200) -> Tuple[torch.Tenso
     ws = torch.empty(int(load().pfd_canny_workspace_bytes(B, H, W)), device=x.device, dtype=torch.uint8)
     out = torch.empty((B, 3, H, W), device=x.device, dtype=torch.float32)
     sweeps = c_int32(0)
-    _check(load().pfd_canny_f32(x.data_ptr(), f32, B, H, W, int(low), int(high),
-                                ws.data_ptr(), out.data_ptr(), ctypes.byref(sweeps), stream_ptr()), "pfd_canny_f32")
+    _call("pfd_canny_f32", x, f32, B, H, W, int(low), int(high), ws, out, ctypes.byref(sweeps))
     return out, int(sweeps.value)
 
 
@@ -672,8 +615,7 @@ def image_u8_roundtrip(x: torch.Tensor) -> torch.Tensor:
         raise RuntimeError("image_u8_roundtrip: expected a CUDA fp16/fp32 tensor")
     x = x.contiguous()
     out = torch.empty(x.shape, device=x.device, dtype=torch.float32)
-    _check(load().pfd_image_u8_roundtrip_f32(x.data_ptr(), int(x.dtype == torch.float32), x.numel(), out.data_ptr(),
-                                             stream_ptr()), "pfd_image_u8_roundtrip_f32")
+    _call("pfd_image_u8_roundtrip_f32", x, int(x.dtype == torch.float32), x.numel(), out)
     return out
 
 
@@ -684,8 +626,7 @@ def hed_input(x: torch.Tensor, norm: torch.Tensor, scale: float, cpad: int = 3) 
     _chk32(norm, "hed_input norm")
     B, _, H, W = x.shape
     out = torch.empty((B, H, W, cpad), device=x.device, dtype=torch.float16)
-    _check(load().pfd_hed_input_f16(x.data_ptr(), f32, B, H, W, cpad, norm.data_ptr(),
-                                    float(scale), out.data_ptr(), stream_ptr()), "pfd_hed_input_f16")
+    _call("pfd_hed_input_f16", x, f32, B, H, W, cpad, norm, float(scale), out)
     return out
 
 
@@ -701,8 +642,7 @@ def hed_pool_side(x: torch.Tensor, proj_w: torch.Tensor, proj_b: torch.Tensor, p
         raise RuntimeError(f"hed_pool_side: proj_w has {proj_w.numel()} entries for C={C}")
     side = torch.empty((B, h, w), device=x.device, dtype=torch.float32)
     pooled = torch.empty((B, h // 2, w // 2, C), device=x.device, dtype=torch.float16) if pool else None
-    _check(load().pfd_hed_pool_side_f16(x.data_ptr(), B, h, w, C, proj_w.data_ptr(), proj_b.data_ptr(),
-                                        side.data_ptr(), _p(pooled), stream_ptr()), "pfd_hed_pool_side_f16")
+    _call("pfd_hed_pool_side_f16", x, B, h, w, C, proj_w, proj_b, side, pooled)
     return side, pooled
 
 
@@ -720,8 +660,7 @@ def hed_fuse(sides: Sequence[torch.Tensor], H: int, W: int, inv_scale: float = 1
     ptrs = (c_void_p * n)(*[s.data_ptr() for s in sides])
     hs = (c_int32 * n)(*[s.shape[1] for s in sides])
     ws = (c_int32 * n)(*[s.shape[2] for s in sides])
-    _check(load().pfd_hed_fuse_f32(ptrs, hs, ws, n, B, H, W, float(inv_scale), out.data_ptr(), stream_ptr()),
-           "pfd_hed_fuse_f32")
+    _call("pfd_hed_fuse_f32", ptrs, hs, ws, n, B, H, W, float(inv_scale), out)
     return out
 
 
@@ -735,8 +674,7 @@ def scribble_hed(hed: torch.Tensor, return_nms: bool = False):
     B, C, H, W = hed.shape
     nms = torch.empty((B, H, W), device=hed.device, dtype=torch.uint8)
     out = torch.empty((B, 3, H, W), device=hed.device, dtype=torch.float32)
-    _check(load().pfd_scribble_hed_f32(hed.data_ptr(), C * H * W, B, H, W, nms.data_ptr(), out.data_ptr(),
-                                       stream_ptr()), "pfd_scribble_hed_f32")
+    _call("pfd_scribble_hed_f32", hed, C * H * W, B, H, W, nms, out)
     return (out, nms) if return_nms else out
 
 
@@ -749,8 +687,7 @@ def scribble_blur_u8(z: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     B, H, W = z.shape
     blurred = torch.empty_like(z)
     out = torch.empty((B, 3, H, W), device=z.device, dtype=torch.float32)
-    _check(load().pfd_scribble_blur_u8(z.data_ptr(), B, H, W, blurred.data_ptr(), out.data_ptr(), stream_ptr()),
-           "pfd_scribble_blur_u8")
+    _call("pfd_scribble_blur_u8", z, B, H, W, blurred, out)
     return blurred, out
 
 
@@ -760,8 +697,7 @@ def scribble_xdog(x: torch.Tensor, threshold: int = 32) -> torch.Tensor:
     x, f32 = _chk_image(x, "scribble_xdog")
     B, _, H, W = x.shape
     out = torch.empty((B, 3, H, W), device=x.device, dtype=torch.float32)
-    _check(load().pfd_scribble_xdog_f32(x.data_ptr(), f32, B, H, W, int(threshold),
-                                        out.data_ptr(), stream_ptr()), "pfd_scribble_xdog_f32")
+    _call("pfd_scribble_xdog_f32", x, f32, B, H, W, int(threshold), out)
     return out
 
 
@@ -779,8 +715,7 @@ def pidinet_dw(x: torch.Tensor, w: torch.Tensor, pool: bool = False):
     h, wd = (H // 2, W // 2) if pool else (H, W)
     out = torch.empty((B, h, wd, C), device=x.device, dtype=torch.float16)
     pooled = torch.empty_like(out) if pool else None
-    _check(load().pfd_pidinet_dw_f16(x.data_ptr(), B, H, W, C, ks, int(pool), w.data_ptr(), out.data_ptr(), _p(pooled),
-                                     stream_ptr()), "pfd_pidinet_dw_f16")
+    _call("pfd_pidinet_dw_f16", x, B, H, W, C, ks, int(pool), w, out, pooled)
     return (out, pooled) if pool else out
 
 
@@ -795,8 +730,7 @@ def pidinet_reduce(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor) -> torch.T
     if tuple(w.shape) != (C, 24) or b.numel() != 24:
         raise RuntimeError(f"pidinet_reduce: weights {tuple(w.shape)} / bias {tuple(b.shape)} do not fit C={C}")
     m = torch.empty((B, h, wd, 24), device=x.device, dtype=torch.float16)
-    _check(load().pfd_pidinet_reduce_f16(x.data_ptr(), B * h * wd, C, w.data_ptr(), b.data_ptr(), m.data_ptr(),
-                                         stream_ptr()), "pfd_pidinet_reduce_f16")
+    _call("pfd_pidinet_reduce_f16", x, B * h * wd, C, w, b, m)
     return m
 
 
@@ -810,8 +744,7 @@ def pidinet_cdcm(m: torch.Tensor, wpk: torch.Tensor) -> torch.Tensor:
     if C != 24 or wpk.numel() != 54 * 3 * 32 * 4:
         raise RuntimeError(f"pidinet_cdcm: m {tuple(m.shape)} / packed weights {wpk.numel()} do not fit")
     u = torch.empty((B, h, w, 24), device=m.device, dtype=torch.float32)
-    _check(load().pfd_pidinet_cdcm_f16(m.data_ptr(), B, h, w, wpk.data_ptr(), u.data_ptr(), stream_ptr()),
-           "pfd_pidinet_cdcm_f16")
+    _call("pfd_pidinet_cdcm_f16", m, B, h, w, wpk, u)
     return u
 
 
@@ -823,8 +756,7 @@ def pidinet_side(u: torch.Tensor, params: torch.Tensor) -> torch.Tensor:
     if C != 24 or params.numel() != PFD_PIDINET_SIDE_PARAMS:
         raise RuntimeError(f"pidinet_side: u {tuple(u.shape)} / params {params.numel()} do not fit")
     side = torch.empty((B, h, w), device=u.device, dtype=torch.float32)
-    _check(load().pfd_pidinet_side_f32(u.data_ptr(), B, h, w, params.data_ptr(), side.data_ptr(), stream_ptr()),
-           "pfd_pidinet_side_f32")
+    _call("pfd_pidinet_side_f32", u, B, h, w, params, side)
     return side
 
 
@@ -843,8 +775,7 @@ def pidinet_fuse(sides: Sequence[torch.Tensor], cls: torch.Tensor, H: int, W: in
     ptrs = (c_void_p * 4)(*[s.data_ptr() for s in sides])
     hs = (c_int32 * 4)(*[s.shape[1] for s in sides])
     ws = (c_int32 * 4)(*[s.shape[2] for s in sides])
-    _check(load().pfd_pidinet_fuse_f32(ptrs, hs, ws, B, H, W, cls.data_ptr(), out.data_ptr(), stream_ptr()),
-           "pfd_pidinet_fuse_f32")
+    _call("pfd_pidinet_fuse_f32", ptrs, hs, ws, B, H, W, cls, out)
     return out
 
 
@@ -854,8 +785,7 @@ def mlsd_input(x: torch.Tensor) -> torch.Tensor:
     x, f32 = _chk_image(x, "mlsd_input")
     B, _, H, W = x.shape
     out = torch.empty((B, H, W, 16), device=x.device, dtype=torch.float16)
-    _check(load().pfd_mlsd_input_f16(x.data_ptr(), f32, B, H, W, out.data_ptr(),
-                                     stream_ptr()), "pfd_mlsd_input_f16")
+    _call("pfd_mlsd_input_f16", x, f32, B, H, W, out)
     return out
 
 
@@ -870,8 +800,7 @@ def mlsd_dw(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, stride: int) -> t
     if tuple(w.shape) != (9, C) or b.numel() != C:
         raise RuntimeError(f"mlsd_dw: weights {tuple(w.shape)} / bias {tuple(b.shape)} do not fit C={C}")
     out = torch.empty((B, H // stride, W // stride, C), device=x.device, dtype=torch.float16)
-    _check(load().pfd_mlsd_dw_f16(x.data_ptr(), B, H, W, C, int(stride), w.data_ptr(), b.data_ptr(), out.data_ptr(),
-                                  stream_ptr()), "pfd_mlsd_dw_f16")
+    _call("pfd_mlsd_dw_f16", x, B, H, W, C, int(stride), w, b, out)
     return out
 
 
@@ -886,8 +815,7 @@ def mlsd_upsample(x: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
     if tuple(out.shape) != (B, 2 * h, 2 * w, C) or out.stride(3) != 1 or out.stride(1) != 2 * w * p \
             or out.stride(0) != 2 * h * out.stride(1):
         raise RuntimeError(f"mlsd_upsample: out {tuple(out.shape)} / strides {out.stride()} do not fit x {tuple(x.shape)}")
-    _check(load().pfd_mlsd_upsample_f16(x.data_ptr(), B, h, w, C, out.data_ptr(), p, stream_ptr()),
-           "pfd_mlsd_upsample_f16")
+    _call("pfd_mlsd_upsample_f16", x, B, h, w, C, out, p)
     return out
 
 
@@ -901,8 +829,7 @@ def mlsd_head(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor) -> torch.Tensor
     if tuple(w.shape) != (5, C) or b.numel() != 5:
         raise RuntimeError(f"mlsd_head: weights {tuple(w.shape)} / bias {tuple(b.shape)} do not fit C={C}")
     out = torch.empty((B, 5, h, wd), device=x.device, dtype=torch.float32)
-    _check(load().pfd_mlsd_head_f32(x.data_ptr(), B, h, wd, C, w.data_ptr(), b.data_ptr(), out.data_ptr(),
-                                    stream_ptr()), "pfd_mlsd_head_f32")
+    _call("pfd_mlsd_head_f32", x, B, h, wd, C, w, b, out)
     return out
 
 
@@ -916,8 +843,7 @@ def mlsd_decode(maps: torch.Tensor, thr_v: float, thr_d: float) -> Tuple[torch.T
     keys = torch.empty((B, h, w), device=maps.device, dtype=torch.int32)
     segs = torch.empty((B, PFD_MLSD_TOPK, 4), device=maps.device, dtype=torch.int32)
     count = torch.empty((B,), device=maps.device, dtype=torch.int32)
-    _check(load().pfd_mlsd_decode_f32(maps.data_ptr(), B, h, w, float(thr_v), float(thr_d), keys.data_ptr(),
-                                      segs.data_ptr(), count.data_ptr(), stream_ptr()), "pfd_mlsd_decode_f32")
+    _call("pfd_mlsd_decode_f32", maps, B, h, w, float(thr_v), float(thr_d), keys, segs, count)
     return segs, count
 
 
@@ -930,8 +856,7 @@ def mlsd_draw(segs: torch.Tensor, count: torch.Tensor, H: int, W: int) -> torch.
     segs, count = segs.contiguous(), count.contiguous()
     B = segs.shape[0]
     out = torch.zeros((B, 3, H, W), device=segs.device, dtype=torch.float32)
-    _check(load().pfd_mlsd_draw_f32(segs.data_ptr(), count.data_ptr(), B, H, W, out.data_ptr(), stream_ptr()),
-           "pfd_mlsd_draw_f32")
+    _call("pfd_mlsd_draw_f32", segs, count, B, H, W, out)
     return out
 
 
@@ -943,8 +868,7 @@ def openpose_input(x: torch.Tensor, h: int, w: int, hp: int, wp: int, plan, tabs
     B, _, H, W = x.shape
     out = torch.empty((B, hp, wp, 16), device=x.device, dtype=torch.float16)
     mode, fy, fx, ay, ax = _plan_args(plan, tabs, u8=True)
-    _check(load().pfd_openpose_input_f16(x.data_ptr(), f32, B, H, W, h, w, hp, wp, mode, fy,
-                                         fx, *ay, *ax, out.data_ptr(), stream_ptr()), "pfd_openpose_input_f16")
+    _call("pfd_openpose_input_f16", x, f32, B, H, W, h, w, hp, wp, mode, fy, fx, *ay, *ax, out)
     return out
 
 
@@ -957,7 +881,7 @@ def _plan_args(plan, tabs, u8: bool = False):
         return 1, plan[1], plan[2], none, none
     (iy, wy), (ix, wx) = tabs
     mode = (2 if wy.dtype == torch.int32 else 3) if u8 else 2
-    return mode, 0, 0, (iy.data_ptr(), wy.data_ptr(), iy.shape[1]), (ix.data_ptr(), wx.data_ptr(), ix.shape[1])
+    return mode, 0, 0, (iy, wy, iy.shape[1]), (ix, wx, ix.shape[1])
 
 
 def openpose_pool(x: torch.Tensor) -> torch.Tensor:
@@ -966,7 +890,7 @@ def openpose_pool(x: torch.Tensor) -> torch.Tensor:
     x = x.contiguous()
     B, H, W, C = x.shape
     out = torch.empty((B, H // 2, W // 2, C), device=x.device, dtype=torch.float16)
-    _check(load().pfd_openpose_pool_f16(x.data_ptr(), B, H, W, C, out.data_ptr(), stream_ptr()), "pfd_openpose_pool_f16")
+    _call("pfd_openpose_pool_f16", x, B, H, W, C, out)
     return out
 
 
@@ -976,7 +900,7 @@ def im2col7x7(x: torch.Tensor) -> torch.Tensor:
     x = x.contiguous()
     B, H, W, C = x.shape
     out = torch.empty((B * H * W, 49 * C), device=x.device, dtype=torch.float16)
-    _check(load().pfd_im2col7x7_f16(x.data_ptr(), B, H, W, C, out.data_ptr(), stream_ptr()), "pfd_im2col7x7_f16")
+    _call("pfd_im2col7x7_f16", x, B, H, W, C, out)
     return out
 
 
@@ -992,8 +916,7 @@ def openpose_head(x: torch.Tensor, w: torch.Tensor, b: torch.Tensor, relu: bool,
     N = w.shape[0]
     if w.shape[1] != C or b.numel() != N or out.shape[0] != B or tuple(out.shape[2:]) != (h, wd):
         raise RuntimeError(f"openpose_head: weights {tuple(w.shape)} / out {tuple(out.shape)} do not fit x {tuple(x.shape)}")
-    _check(load().pfd_openpose_head_f32(x.data_ptr(), B, h, wd, C, w.data_ptr(), b.data_ptr(), N, int(relu),
-                                        out.data_ptr(), out.shape[1], off, stream_ptr()), "pfd_openpose_head_f32")
+    _call("pfd_openpose_head_f32", x, B, h, wd, C, w, b, N, int(relu), out, out.shape[1], off)
 
 
 def openpose_resize(src: torch.Tensor, c0: int, C: int, H: int, W: int, plan, tabs) -> torch.Tensor:
@@ -1003,8 +926,7 @@ def openpose_resize(src: torch.Tensor, c0: int, C: int, H: int, W: int, plan, ta
     B, Cs, hs, ws = src.shape
     out = torch.empty((B, C, H, W), device=src.device, dtype=torch.float32)
     mode, fy, fx, ay, ax = _plan_args(plan, tabs)
-    _check(load().pfd_openpose_resize_f32(src.data_ptr(), B, Cs, c0, C, hs, ws, H, W, mode, fy, fx, *ay, *ax,
-                                          out.data_ptr(), stream_ptr()), "pfd_openpose_resize_f32")
+    _call("pfd_openpose_resize_f32", src, B, Cs, c0, C, hs, ws, H, W, mode, fy, fx, *ay, *ax, out)
     return out
 
 
@@ -1022,9 +944,7 @@ def openpose_peaks(maps: torch.Tensor, gauss: torch.Tensor):
     xy = torch.zeros((B, 18, PFD_OPENPOSE_MAX_PEAKS, 2), device=dev, dtype=torch.int32)
     score = torch.zeros((B, 18, PFD_OPENPOSE_MAX_PEAKS), device=dev, dtype=torch.float64)
     total = torch.empty((B, 18), device=dev, dtype=torch.int32)
-    _check(load().pfd_openpose_peaks_f32(maps.data_ptr(), B, H, W, gauss.data_ptr(), tmp.data_ptr(), blur.data_ptr(),
-                                         rowcnt.data_ptr(), xy.data_ptr(), score.data_ptr(), total.data_ptr(),
-                                         stream_ptr()), "pfd_openpose_peaks_f32")
+    _call("pfd_openpose_peaks_f32", maps, B, H, W, gauss, tmp, blur, rowcnt, xy, score, total)
     return xy, score, total
 
 
@@ -1042,10 +962,8 @@ def openpose_assemble(up: torch.Tensor, H: int, W: int, plan, tabs, total: torch
     pscore = torch.empty((B, R, 2), device=dev, dtype=torch.float64)
     npersons = torch.empty((B,), device=dev, dtype=torch.int32)
     mode, fy, fx, ay, ax = _plan_args(plan, tabs)
-    _check(load().pfd_openpose_assemble_f32(up.data_ptr(), B, C, hs, ws, H, W, mode, fy, fx, *ay, *ax, total.data_ptr(),
-                                            xy.data_ptr(), score.data_ptr(), conn.data_ptr(), rows.data_ptr(),
-                                            persons.data_ptr(), pscore.data_ptr(), npersons.data_ptr(), stream_ptr()),
-           "pfd_openpose_assemble_f32")
+    _call("pfd_openpose_assemble_f32", up, B, C, hs, ws, H, W, mode, fy, fx, *ay, *ax, total, xy, score, conn, rows,
+          persons, pscore, npersons)
     return persons, pscore, npersons
 
 
@@ -1056,9 +974,7 @@ def openpose_draw(persons: torch.Tensor, npersons: torch.Tensor, xy: torch.Tenso
     dev = persons.device
     idx = torch.empty((B, H, W), device=dev, dtype=torch.int32)
     out = torch.empty((B, 3, H, W), device=dev, dtype=torch.float32)
-    _check(load().pfd_openpose_draw_f32(persons.data_ptr(), npersons.data_ptr(), xy.data_ptr(), B, H, W,
-                                        sintab.data_ptr(), colors.data_ptr(), idx.data_ptr(), out.data_ptr(),
-                                        stream_ptr()), "pfd_openpose_draw_f32")
+    _call("pfd_openpose_draw_f32", persons, npersons, xy, B, H, W, sintab, colors, idx, out)
     return out
 
 
@@ -1066,8 +982,7 @@ def window_gather(x: torch.Tensor, ws: int, shift: int) -> torch.Tensor:
     B, H, W, C = x.shape
     Hp, Wp = -(-H // ws) * ws, -(-W // ws) * ws
     out = torch.empty((B * (Hp // ws) * (Wp // ws), ws * ws, C), device=x.device, dtype=torch.float16)
-    _check(load().pfd_window_gather_f16(x.data_ptr(), B, H, W, C, ws, shift, out.data_ptr(), stream_ptr()),
-           "pfd_window_gather_f16")
+    _call("pfd_window_gather_f16", x, B, H, W, C, ws, shift, out)
     return out
 
 
@@ -1075,16 +990,14 @@ def window_scatter(win: torch.Tensor, B: int, H: int, W: int, ws: int, shift: in
                    residual: Optional[torch.Tensor]) -> torch.Tensor:
     C = win.shape[-1]
     out = torch.empty((B, H, W, C), device=win.device, dtype=torch.float16)
-    _check(load().pfd_window_scatter_f16(win.data_ptr(), B, H, W, C, ws, shift, _p(residual),
-                                         out.data_ptr(), stream_ptr()), "pfd_window_scatter_f16")
+    _call("pfd_window_scatter_f16", win, B, H, W, C, ws, shift, residual, out)
     return out
 
 
 def patch_merge_gather(x: torch.Tensor) -> torch.Tensor:
     B, H, W, C = x.shape
     out = torch.empty((B, (H + 1) // 2, (W + 1) // 2, 4 * C), device=x.device, dtype=torch.float16)
-    _check(load().pfd_patch_merge_gather_f16(x.data_ptr(), B, H, W, C, out.data_ptr(), stream_ptr()),
-           "pfd_patch_merge_gather_f16")
+    _call("pfd_patch_merge_gather_f16", x, B, H, W, C, out)
     return out
 
 
@@ -1095,8 +1008,7 @@ def patchify(img: torch.Tensor, P: int, kpad: int) -> torch.Tensor:
     if img.dtype not in (torch.float16, torch.float32):
         img = img.to(torch.float16)
     out = torch.empty((B, -(-H // P), -(-W // P), kpad), device=img.device, dtype=torch.float16)
-    _check(load().pfd_patchify_f16(img.data_ptr(), int(img.dtype == torch.float32), B, C, H, W, P, kpad,
-                                   out.data_ptr(), stream_ptr()), "pfd_patchify_f16")
+    _call("pfd_patchify_f16", img, int(img.dtype == torch.float32), B, C, H, W, P, kpad, out)
     return out
 
 
@@ -1132,9 +1044,8 @@ def flash_attn(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, *, B: int, he
     d = q.shape[2]
     _check_flash_shapes("flash_attn", q.shape[1], k.shape[1], k.shape[2], vt.shape[1], vt.shape[2], d, Nq, Nk)
     _check_flash_out("flash_attn", out, B, heads, Nq, d)
-    _check(load().pfd_flash_attn_f16(q.data_ptr(), k.data_ptr(), vt.data_ptr(), out.data_ptr(), B, heads, Nq, Nk,
-                                     d, q.shape[1], k.shape[1], scale, vt.shape[2], out.stride(0), out.stride(1),
-                                     0, stream_ptr()), "pfd_flash_attn_f16")
+    _call("pfd_flash_attn_f16", q, k, vt, out, B, heads, Nq, Nk, d, q.shape[1], k.shape[1], scale, vt.shape[2],
+          out.stride(0), out.stride(1), 0)
     return out
 
 
@@ -1151,7 +1062,6 @@ def flash_attn_strided(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, *, Nq
     _check_flash_shapes("flash_attn_strided", q.shape[2], k.shape[2], k.shape[3], vt.shape[2], vt.shape[3], d, Nq, Nk)
     _check_flash_out("flash_attn_strided", out, B, heads, Nq, d)
     st = lambda t: (c_int64 * 3)(t.stride(0), t.stride(1), t.stride(2))
-    _check(load().pfd_flash_attn_strided_f16(q.data_ptr(), k.data_ptr(), vt.data_ptr(), out.data_ptr(), B, heads, Nq,
-                                             Nk, d, st(q), st(k), st(vt), scale, out.stride(0), out.stride(1),
-                                             stream_ptr()), "pfd_flash_attn_strided_f16")
+    _call("pfd_flash_attn_strided_f16", q, k, vt, out, B, heads, Nq, Nk, d, st(q), st(k), st(vt), scale, out.stride(0),
+          out.stride(1))
     return out

@@ -220,8 +220,7 @@ class PiDiNet(nn.Module):
             raise ValueError(f"PiDiNet needs H and W >= {MIN_SIZE} (three 2x2 floor pools), got {H}x{W}")
         init, blocks, stages, cls, zeros = self._packed()
         h = nv.hed_input(x, zeros, 1.0)                      # u8 levels, exact in fp16 (u8 / 255 would round)
-        col = nv.im2col3x3(h, init.shape[1])
-        h = nv.linear(col.reshape(B * H * W, init.shape[1]), init).reshape(B, H, W, init.shape[0])
+        h = nv.conv3x3_im2col(h, init)
         feats = []
         for wd, w2, bias, stride in blocks:
             if stride > 1:

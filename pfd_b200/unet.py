@@ -356,10 +356,8 @@ class UNetModel2D_Next(nn.Module):
             w, bb = pk_conv3(layer[2])                                # rows padded to 8 output channels
             return nv.conv3x3(hn, w, bb)
         if isinstance(layer, Conv2d):                                 # stem conv, Cin=4: im2col path
-            w, b, kpad = pk_conv3_small(layer)
-            B, H, W, _ = h.shape
-            col = nv.im2col3x3(h, kpad)
-            return nv.linear(col.reshape(B * H * W, kpad), w, b).reshape(B, H, W, w.shape[0])
+            w, b = pk_conv3_small(layer)
+            return nv.conv3x3_im2col(h, w, b)
         raise RuntimeError(f"unknown data block {type(layer)}")
 
     def apply(self, x: torch.Tensor, timesteps: torch.Tensor, context: torch.Tensor,
