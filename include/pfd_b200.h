@@ -495,6 +495,37 @@ PFD_API int pfd_openpose_draw_f32(const int32_t* persons, const int32_t* nperson
                                   int32_t H, int32_t W, const float* sintab, const uint8_t* colors, int32_t* idx,
                                   float* out, void* stream);
 
+/* OpenPose face annotator, ControlNet.preprocess(type='openpose_withface' / 'openpose_withface_v11p')
+ * (controlnet.py:408-418 -> OpenposeDetector(include_face=True): util.faceDetect, Face.__call__,
+ * Face.compute_peaks_from_heatmaps and util.draw_facepose), on top of the body annotator above.  FaceNet's convs run on
+ * pfd_gemm_f16, pfd_im2col7x7_f16, pfd_openpose_pool_f16 and pfd_openpose_head_f32.
+ * pfd_openpose_face_boxes: util.faceDetect (float64) of every person of pfd_openpose_assemble_f32's output: boxes int32
+ *   [B*MAX_PERSONS, 6] = (image, person, x, y, ch, cw) of the crop oriImg[y:y+w, x:x+w] as numpy clips it, compacted
+ *   in (image, person) order; count int32 [1] = the number of boxes.
+ * pfd_openpose_face_input_f16: one face's network input, out channel-last fp16 [D,D,16]: the crop (cx, cy, ch x cw)
+ *   of image n (ToPILImage quantisation, BGR), cv2.resize to D x D (mode 0 copy, 1 block mean fy x fx, 2 uint8
+ *   LANCZOS4, 3 INTER_AREA with float weights, 4 INTER_AREA emulated by OpenCV's uint8 bilinear (2 taps, int weights)),
+ *   u8 / 256 - 0.5; channels 3..15 are zero.  Tables as in pfd_openpose_input_f16 (openpose_tables.resize_plan).
+ * pfd_openpose_face_peaks_f32: maps fp32 [F,C,hs,ws] (C = 71) -> lmk int32 [F,C,2]: per channel the first maximum in
+ *   raster order of F.interpolate(maps, (ch, cw), bilinear, align_corners=True) among values > 0.05, as (x, y) in the
+ *   crop of boxes[f] (int32 [F,6] as written by pfd_openpose_face_boxes), or (-1, -1) when no value passes.
+ * pfd_openpose_face_draw_f32: draw_poses with the body and face of every person on a zero canvas: per person its
+ *   body primitives (as pfd_openpose_draw_f32), then its face's landmarks (float32 normalisation, int(x * W), drawn
+ *   where x, y > 0.01) as white cv2.circle(r=3).  colors uint8 [106,3]: the 35 body colours, then 71 x white.
+ */
+PFD_API int pfd_openpose_face_boxes(const int32_t* persons, const int32_t* npersons, const int32_t* xy, int32_t B,
+                                    int32_t H, int32_t W, int32_t* boxes, int32_t* count, void* stream);
+PFD_API int pfd_openpose_face_input_f16(const void* x, int32_t x_f32, int32_t B, int32_t H, int32_t W, int32_t n,
+                                        int32_t cx, int32_t cy, int32_t ch, int32_t cw, int32_t D, int32_t mode,
+                                        int32_t fy, int32_t fx, const int32_t* iy, const void* wy, int32_t ty,
+                                        const int32_t* ix, const void* wx, int32_t tx, void* out, void* stream);
+PFD_API int pfd_openpose_face_peaks_f32(const float* maps, int32_t F, int32_t C, int32_t hs, int32_t ws,
+                                        const int32_t* boxes, int32_t* lmk, void* stream);
+PFD_API int pfd_openpose_face_draw_f32(const int32_t* persons, const int32_t* npersons, const int32_t* xy, int32_t B,
+                                       int32_t H, int32_t W, const float* sintab, const uint8_t* colors,
+                                       const int32_t* boxes, const int32_t* lmk, int32_t F, int32_t* idx, float* out,
+                                       void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -170,10 +170,14 @@ class ControlNet(nn.Module):
         method='xdog' (threshold=32), see scribble.py, and 'mlsd' / 'mlsd_v11p' (the M-LSD line network and its
         decode, thr_v=0.1, thr_d=0.1; weights from pfd_b200.mlsd.load_mlsd / set_network, see mlsd.py) and 'openpose' /
         'openpose_v11p' (the OpenPose body network, its decode and drawing; weights from
-        pfd_b200.openpose.load_openpose / set_network, see openpose.py).  x: [B,3,H,W] tensor in [0,1] or an image path.
+        pfd_b200.openpose.load_openpose / set_network, see openpose.py) and 'openpose_withface' /
+        'openpose_withface_v11p' (the body annotator, then the OpenPose face network on each person's face box, its
+        landmarks and the face dots; face weights from pfd_b200.openpose_face.load_face / set_network, see
+        openpose_face.py; this type reads the face count back to the host once per call and cannot be captured in a
+        CUDA graph).  x: [B,3,H,W] tensor in [0,1] or an image path.
         Returns float32 [B,3,H,W] on x's device; `size=` is ignored, as in the reference.  The other annotators (midas,
-        openpose with face / hand) raise NotImplementedError, and so do method='pidinet', 'mlsd' and 'openpose' while
-        their weights are not installed; an unknown scribble method raises ValueError."""
+        openpose with hands) raise NotImplementedError, and so do method='pidinet', 'mlsd', 'openpose' and
+        'openpose_withface' while their weights are not installed; an unknown scribble method raises ValueError."""
         if type == "none" or type is None:
             return None
         if isinstance(x, str):
@@ -208,9 +212,13 @@ class ControlNet(nn.Module):
         if type in ("openpose", "openpose_v11p"):
             from .openpose import preprocess_openpose
             return preprocess_openpose(x)
+        if type in ("openpose_withface", "openpose_withface_v11p"):
+            from .openpose_face import preprocess_openpose_face
+            return preprocess_openpose_face(x)
         if type is not None and type.startswith("openpose_with"):
-            raise NotImplementedError(f"controlnet annotator '{type}' needs the OpenPose hand / face networks, which "
-                                      "pfd_b200 does not implement; type='openpose' runs the body annotator on the GPU")
+            raise NotImplementedError(f"controlnet annotator '{type}' needs the OpenPose hand network, which pfd_b200 "
+                                      "does not implement; type='openpose' runs the body annotator and "
+                                      "'openpose_withface' the body and face annotators on the GPU")
         raise NotImplementedError(f"controlnet annotator '{type}' is not implemented in pfd_b200 (the GPU serves "
                                   "'input', 'canny', 'hed', 'scribble', 'mlsd' and 'openpose'); feed a ready control "
                                   "map (do_preprocess=False)")

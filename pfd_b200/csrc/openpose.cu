@@ -22,6 +22,14 @@
 //   op_draw_kernel      one warp per primitive: cv2.ellipse2Poly + fillConvexPoly (shift 0, LINE_8) per limb and the
 //                       filled cv2.circle(r=4) per keypoint; the last primitive in drawing order wins each pixel
 //                       (atomicMax of the primitive's index), then op_color_kernel writes the canvas / 255.
+// The face annotator ('openpose_withface', util.faceDetect / Face / draw_facepose) adds:
+//   op_face_boxes_kernel   faceDetect of every person in float64, compacted in (image, person) order by a block scan;
+//   op_face_input_kernel   one face's crop, smart_resize to 384 x 384 (op_resize_u8, including OpenCV's bilinear
+//                          emulation of INTER_AREA when a crop side is below 384), u8 / 256 - 0.5;
+//   op_face_peaks_kernel   one CTA per (face, channel): the align_corners bilinear map at every crop pixel in fp32, the
+//                          first maximum above 0.05 in raster order;
+//   op_face_dots_kernel    float32 normalisation and cv2.circle(r=3) per landmark, drawn after its person's body
+//                          (op_draw_kernel<OP_FACE_PRIMS> spaces each person's primitives 106 apart).
 // Every kernel computes an image's values from that image only, so a batch gives the same bits as single images.  No
 // count leaves the device.
 #include <cuda_fp16.h>
@@ -58,8 +66,61 @@ struct OpAxis {
 template <typename T>
 __device__ __forceinline__ int op_u8(const T* x, long long off) { return (int)to_u8<T>(x[off]); }
 
-// out[n, y, x, 0..15] for the padded network input.  mode 0: copy, 1: integer block mean (fy x fx), 2: LANCZOS4
-// (int16 weights, int sums, (v + 2^21) >> 22), 3: INTER_AREA (float weights, sum, cvRound).
+// cv2.resize of a uint8 plane at output pixel (Y, X); src points at the plane's (crop's) top-left element, ld is its
+// row pitch.  mode 0: copy, 1: integer block mean (fy x fx), 2: LANCZOS4 (int16 weights, int sums,
+// (v + 2^21) >> 22), 3: INTER_AREA (float weights, sum, cvRound), 4: INTER_AREA emulated by OpenCV's uint8 bilinear
+// (2 taps, int16 weights, VResizeLinear's ((b0 * (r0 >> 4)) >> 16) + ((b1 * (r1 >> 4)) >> 16) + 2) >> 2).
+template <typename T>
+__device__ __forceinline__ int op_resize_u8(const T* __restrict__ src, long long ld, int mode, int fy, int fx,
+                                            const OpAxis& ay, const OpAxis& ax, int Y, int X) {
+  if (mode == 0) return op_u8(src, (long long)Y * ld + X);
+  if (mode == 1) {
+    int s = 0;
+    for (int a = 0; a < fy; ++a)
+      for (int b = 0; b < fx; ++b) s += op_u8(src, (long long)(Y * fy + a) * ld + X * fx + b);
+    if (fy == 2 && fx == 2) return (s + 2) >> 2;
+    return min(max(__float2int_rn(__fmul_rn((float)s, 1.f / (float)(fy * fx))), 0), 255);
+  }
+  if (mode == 2) {
+    const int* iy = ay.idx + Y * 8;
+    const int* ix = ax.idx + X * 8;
+    const int* wy = static_cast<const int*>(ay.w) + Y * 8;
+    const int* wx = static_cast<const int*>(ax.w) + X * 8;
+    int acc = 0;
+    for (int k = 0; k < 8; ++k) {
+      int row = 0;
+      for (int j = 0; j < 8; ++j) row += op_u8(src, (long long)iy[k] * ld + ix[j]) * wx[j];
+      acc += row * wy[k];
+    }
+    return min(max((acc + (1 << 21)) >> 22, 0), 255);
+  }
+  if (mode == 4) {
+    const int* iy = ay.idx + Y * 2;
+    const int* ix = ax.idx + X * 2;
+    const int* wy = static_cast<const int*>(ay.w) + Y * 2;
+    const int* wx = static_cast<const int*>(ax.w) + X * 2;
+    int r[2];
+    for (int k = 0; k < 2; ++k) {
+      const long long row = (long long)iy[k] * ld;
+      r[k] = op_u8(src, row + ix[0]) * wx[0] + op_u8(src, row + ix[1]) * wx[1];
+    }
+    return min(max((((wy[0] * (r[0] >> 4)) >> 16) + ((wy[1] * (r[1] >> 4)) >> 16) + 2) >> 2, 0), 255);
+  }
+  const int* iy = ay.idx + Y * ay.taps;
+  const int* ix = ax.idx + X * ax.taps;
+  const float* wy = static_cast<const float*>(ay.w) + Y * ay.taps;
+  const float* wx = static_cast<const float*>(ax.w) + X * ax.taps;
+  float acc = 0.f;
+  for (int k = 0; k < ay.taps; ++k) {
+    float row = 0.f;
+    for (int j = 0; j < ax.taps; ++j)
+      row = __fadd_rn(row, __fmul_rn((float)op_u8(src, (long long)iy[k] * ld + ix[j]), wx[j]));
+    acc = __fadd_rn(acc, __fmul_rn(wy[k], row));
+  }
+  return min(max(__float2int_rn(acc), 0), 255);
+}
+
+// out[n, y, x, 0..15] for the padded network input (modes 0-3 of op_resize_u8)
 template <typename T>
 __global__ void __launch_bounds__(256)
 op_input_kernel(const T* __restrict__ x, int B, int H, int W, int h, int w, int hp, int wp, int mode, int fy, int fx,
@@ -78,42 +139,7 @@ op_input_kernel(const T* __restrict__ x, int B, int H, int W, int h, int w, int 
     if (Y < h && X < w) {
 #pragma unroll
       for (int c = 0; c < 3; ++c) {
-        const long long base = (n * 3 + (2 - c)) * hw;      // BGR
-        int u = 0;
-        if (mode == 0) {
-          u = op_u8(x, base + (long long)Y * W + X);
-        } else if (mode == 1) {
-          int s = 0;
-          for (int a = 0; a < fy; ++a)
-            for (int b = 0; b < fx; ++b) s += op_u8(x, base + (long long)(Y * fy + a) * W + X * fx + b);
-          if (fy == 2 && fx == 2) u = (s + 2) >> 2;
-          else u = min(max(__float2int_rn(__fmul_rn((float)s, 1.f / (float)(fy * fx))), 0), 255);
-        } else if (mode == 2) {
-          const int* iy = ay.idx + Y * 8;
-          const int* ix = ax.idx + X * 8;
-          const int* wy = static_cast<const int*>(ay.w) + Y * 8;
-          const int* wx = static_cast<const int*>(ax.w) + X * 8;
-          int acc = 0;
-          for (int k = 0; k < 8; ++k) {
-            int row = 0;
-            for (int j = 0; j < 8; ++j) row += op_u8(x, base + (long long)iy[k] * W + ix[j]) * wx[j];
-            acc += row * wy[k];
-          }
-          u = min(max((acc + (1 << 21)) >> 22, 0), 255);
-        } else {
-          const int* iy = ay.idx + Y * ay.taps;
-          const int* ix = ax.idx + X * ax.taps;
-          const float* wy = static_cast<const float*>(ay.w) + Y * ay.taps;
-          const float* wx = static_cast<const float*>(ax.w) + X * ax.taps;
-          float acc = 0.f;
-          for (int k = 0; k < ay.taps; ++k) {
-            float row = 0.f;
-            for (int j = 0; j < ax.taps; ++j)
-              row = __fadd_rn(row, __fmul_rn((float)op_u8(x, base + (long long)iy[k] * W + ix[j]), wx[j]));
-            acc = __fadd_rn(acc, __fmul_rn(wy[k], row));
-          }
-          u = min(max(__float2int_rn(acc), 0), 255);
-        }
+        const int u = op_resize_u8(x + (n * 3 + (2 - c)) * hw, W, mode, fy, fx, ay, ax, Y, X);   // BGR
         v[c] = __float2half_rn((float)u * (1.f / 256.f) - 0.5f);
       }
     }
@@ -536,11 +562,34 @@ __device__ __forceinline__ void op_put(int* idx, int H, int W, long long x, long
 constexpr int OP_WARPS = 4;
 constexpr int OP_DRAW_BLOCKS = 64;   // per image: 256 warps share the primitives
 
-// One primitive, drawn by one warp: its pixels get atomicMax(prim).  pts: the warp's ellipse2Poly buffer.
+// cv2.circle(r=R, filled), drawn by one warp: the spans of OpenCV's Circle() for radius R get atomicMax(val)
+template <int R>
+__device__ __forceinline__ void op_circle(int* canvas, int H, int W, long long cx, long long cy, int val, int lane) {
+  int err = 0, dx = R, dy = 0, plus = 1, minus = 2 * R - 1;
+  while (dx >= dy) {
+    for (int t = lane; t < 4 * (2 * R + 1); t += 32) {
+      const int span = t / (2 * R + 1), o = t % (2 * R + 1) - R;
+      const int half = span < 2 ? dx : dy, yo = span == 0 ? -dy : span == 1 ? dy : span == 2 ? -dx : dx;
+      if (o >= -half && o <= half) op_put(canvas, H, W, cx + o, cy + yo, val);
+    }
+    dy++;
+    err += plus;
+    plus += 2;
+    const int mask = (err <= 0) - 1;
+    err -= minus & mask;
+    dx += mask;
+    minus -= mask & 2;
+  }
+}
+
+// One primitive, drawn by one warp: its pixels get atomicMax of its drawing-order value (person p's slot s is
+// p * STRIDE + s: STRIDE = OP_PRIMS for the body alone, OP_FACE_PRIMS when face dots follow each person's body).
+// pts: the warp's ellipse2Poly buffer.
+template <int STRIDE>
 __device__ void op_draw_prim(const int* __restrict__ persons, const int* __restrict__ xy, int H, int W,
                              const float* __restrict__ sintab, int* __restrict__ idx, int (*pts)[2], int n, int prim,
                              int lane) {
-  const int p = prim / OP_PRIMS, s = prim % OP_PRIMS;
+  const int p = prim / OP_PRIMS, s = prim % OP_PRIMS, val = p * STRIDE + s;
   const int* person = persons + ((long long)n * OP_ROWS + p) * 18;
   int* canvas = idx + (long long)n * H * W;
   const double fW = W, fH = H;
@@ -556,23 +605,7 @@ __device__ void op_draw_prim(const int* __restrict__ persons, const int* __restr
   if (s >= 17) {
     double kx, ky;
     if (!kp(s - 17, kx, ky)) return;
-    const long long cx = (long long)kx, cy = (long long)ky;
-    // cv2.circle(r=4, filled): the spans of OpenCV's Circle() for radius 4
-    int err = 0, dx = 4, dy = 0, plus = 1, minus = 7;
-    while (dx >= dy) {
-      for (int t = lane; t < 4 * 9; t += 32) {
-        const int span = t / 9, o = t % 9 - 4;
-        const int half = span < 2 ? dx : dy, yo = span == 0 ? -dy : span == 1 ? dy : span == 2 ? -dx : dx;
-        if (o >= -half && o <= half) op_put(canvas, H, W, cx + o, cy + yo, prim);
-      }
-      dy++;
-      err += plus;
-      plus += 2;
-      const int mask = (err <= 0) - 1;
-      err -= minus & mask;
-      dx += mask;
-      minus -= mask & 2;
-    }
+    op_circle<4>(canvas, H, W, (long long)kx, (long long)ky, val, lane);
     return;
   }
   double x1, y1, x2, y2;
@@ -632,7 +665,7 @@ __device__ void op_draw_prim(const int* __restrict__ persons, const int* __restr
   for (int i = 0; i < np; ++i) {
     const int a = i == 0 ? np - 1 : i - 1;
     for_each_line_pixel(W, H, pts[a][0], pts[a][1], pts[i][0], pts[i][1], lane,
-                        [&](long long x, long long y) { atomicMax(canvas + y * W + x, prim); });
+                        [&](long long x, long long y) { atomicMax(canvas + y * W + x, val); });
   }
   long long xmin = pts[0][0], xmax = pts[0][0], ymin = pts[0][1], ymax = pts[0][1];
   int imin = 0;
@@ -678,7 +711,7 @@ __device__ void op_draw_prim(const int* __restrict__ persons, const int* __restr
       if (xx2 >= 0 && xx1 < W) {
         xx1 = max(xx1, 0LL);
         xx2 = min(xx2, (long long)W - 1);
-        for (long long x = xx1 + lane; x <= xx2; x += 32) op_put(canvas, H, W, x, y, prim);
+        for (long long x = xx1 + lane; x <= xx2; x += 32) op_put(canvas, H, W, x, y, val);
       }
     }
     e_x[0] += e_dx[0];
@@ -688,6 +721,7 @@ __device__ void op_draw_prim(const int* __restrict__ persons, const int* __restr
 
 // Warps loop over the primitives of the image's persons (blockIdx.y = image): person p = prim / 35, slot s = prim % 35
 // (limb s < 17, else keypoint s - 17); the grid does not depend on the person count, which stays on the device.  idx: int32 [B, H, W], -1 where nothing is drawn.
+template <int STRIDE>
 __global__ void __launch_bounds__(OP_WARPS * 32)
 op_draw_kernel(const int* __restrict__ persons, const int* __restrict__ npersons, const int* __restrict__ xy, int H,
                int W, const float* __restrict__ sintab, int* __restrict__ idx) {
@@ -696,10 +730,11 @@ op_draw_kernel(const int* __restrict__ persons, const int* __restrict__ npersons
   const int n = blockIdx.y, warp = threadIdx.x / 32, lane = threadIdx.x & 31;
   const int nprim = npersons[n] * OP_PRIMS;
   for (int prim = blockIdx.x * OP_WARPS + warp; prim < nprim; prim += gridDim.x * OP_WARPS)
-    op_draw_prim(persons, xy, H, W, sintab, idx, s_pts[warp], n, prim, lane);
+    op_draw_prim<STRIDE>(persons, xy, H, W, sintab, idx, s_pts[warp], n, prim, lane);
 }
 
-// out[n, c, y, x] = colour[idx % 35][c] / 255 (0 where idx < 0)
+// out[n, c, y, x] = colour[idx % STRIDE][c] / 255 (0 where idx < 0)
+template <int STRIDE>
 __global__ void __launch_bounds__(256)
 op_color_kernel(const int* __restrict__ idx, int B, int H, int W, const unsigned char* __restrict__ colors,
                 float* __restrict__ out) {
@@ -710,7 +745,176 @@ op_color_kernel(const int* __restrict__ idx, int B, int H, int W, const unsigned
     const long long n = i / HW, p = i % HW;
 #pragma unroll
     for (int c = 0; c < 3; ++c)
-      out[(n * 3 + c) * HW + p] = v < 0 ? 0.f : __fdiv_rn((float)colors[(v % OP_PRIMS) * 3 + c], 255.f);
+      out[(n * 3 + c) * HW + p] = v < 0 ? 0.f : __fdiv_rn((float)colors[(v % STRIDE) * 3 + c], 255.f);
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Face annotator (openpose_withface: util.faceDetect, Face.__call__, compute_peaks_from_heatmaps, draw_facepose)
+constexpr int OP_FACE_MAPS = 71;                     // FaceNet's heatmaps, the background channel included
+constexpr int OP_FACE_PRIMS = OP_PRIMS + OP_FACE_MAPS;  // per person: the body's 35 primitives, then 71 face dots
+constexpr int OP_BOX_THREADS = 1024;
+
+// util.faceDetect of person p of image n in float64: false when there is no box, else the crop (x, y, ch, cw) of
+// oriImg[y:y+w, x:x+w] (numpy clips the slice at the image's right and bottom edges)
+__device__ bool op_face_box(const int* __restrict__ person, const int* __restrict__ xy, int n, int H, int W, int* box) {
+  auto kp = [&](int part, double& kx, double& ky) -> bool {
+    const int c = person[part];
+    if (c < 0) return false;
+    const int* q = xy + ((long long)(n * 18 + part) * OP_CAP + c) * 2;
+    kx = q[0], ky = q[1];
+    return true;
+  };
+  double x0, y0, x1, y1;
+  if (!kp(0, x0, y0)) return false;
+  bool any = false;
+  double width = 0.0;
+  for (int part = 14; part < 18; ++part) {
+    if (!kp(part, x1, y1)) continue;
+    any = true;
+    const double d = fmax(fabs(__dsub_rn(x0, x1)), fabs(__dsub_rn(y0, y1)));
+    width = fmax(width, __dmul_rn(d, part < 16 ? 3.0 : 1.5));
+  }
+  if (!any) return false;
+  double x = fmax(__dsub_rn(x0, width), 0.0), y = fmax(__dsub_rn(y0, width), 0.0);
+  double w1 = __dmul_rn(width, 2.0), w2 = w1;
+  if (__dadd_rn(x, width) > (double)W) w1 = __dsub_rn((double)W, x);
+  if (__dadd_rn(y, width) > (double)H) w2 = __dsub_rn((double)H, y);
+  width = fmin(w1, w2);
+  if (!(width >= 20.0)) return false;
+  const int bx = (int)x, by = (int)y, bw = (int)width;
+  box[0] = bx, box[1] = by, box[2] = min(by + bw, H) - by, box[3] = min(bx + bw, W) - bx;
+  return true;
+}
+
+// One CTA: boxes int32 [B * OP_ROWS, 6] = (image, person, x, y, ch, cw) of every person with a face box, compacted
+// in (image, person) order by a block scan; count[0] = their number.
+__global__ void __launch_bounds__(OP_BOX_THREADS)
+op_face_boxes_kernel(const int* __restrict__ persons, const int* __restrict__ npersons, const int* __restrict__ xy,
+                     int B, int H, int W, int* __restrict__ boxes, int* __restrict__ count) {
+  __shared__ int s_scan[OP_BOX_THREADS];
+  pdl_enter();
+  const int tid = threadIdx.x;
+  const long long items = (long long)B * OP_ROWS;
+  int base = 0;
+  for (long long i0 = 0; i0 < items; i0 += OP_BOX_THREADS) {
+    const long long i = i0 + tid;
+    int box[4];
+    const int n = (int)(i / OP_ROWS), p = (int)(i % OP_ROWS);
+    const bool has = i < items && p < npersons[n] &&
+                     op_face_box(persons + ((long long)n * OP_ROWS + p) * 18, xy, n, H, W, box);
+    s_scan[tid] = has;
+    __syncthreads();
+    for (int o = 1; o < OP_BOX_THREADS; o <<= 1) {     // inclusive Hillis-Steele scan
+      const int v = tid >= o ? s_scan[tid - o] : 0;
+      __syncthreads();
+      s_scan[tid] += v;
+      __syncthreads();
+    }
+    if (has) {
+      int* b = boxes + (long long)(base + s_scan[tid] - 1) * 6;
+      b[0] = n, b[1] = p, b[2] = box[0], b[3] = box[1], b[4] = box[2], b[5] = box[3];
+    }
+    base += s_scan[OP_BOX_THREADS - 1];
+    __syncthreads();
+  }
+  if (tid == 0) count[0] = base;
+}
+
+// out[Y, X, 0..15] (D x D, channel-last) of one face: its crop of image n, cv2.resize by op_resize_u8, BGR,
+// u8 / 256 - 0.5 (channels 3..15 zero)
+template <typename T>
+__global__ void __launch_bounds__(256)
+op_face_input_kernel(const T* __restrict__ x, int H, int W, int n, int cx, int cy, int D, int mode, int fy, int fx,
+                     OpAxis ay, OpAxis ax, __half* __restrict__ out) {
+  pdl_enter();
+  const long long hw = (long long)H * W, total = (long long)D * D;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const int X = (int)(i % D), Y = (int)(i / D);
+    __align__(16) __half v[16];
+#pragma unroll
+    for (int c = 0; c < 16; ++c) v[c] = __float2half_rn(0.f);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const T* crop = x + ((long long)n * 3 + (2 - c)) * hw + (long long)cy * W + cx;
+      v[c] = __float2half_rn((float)op_resize_u8(crop, W, mode, fy, fx, ay, ax, Y, X) * (1.f / 256.f) - 0.5f);
+    }
+    uint4* o = reinterpret_cast<uint4*>(out + i * OP_CIN);
+    o[0] = reinterpret_cast<const uint4*>(v)[0];
+    o[1] = reinterpret_cast<const uint4*>(v)[1];
+  }
+}
+
+// torch's align_corners bilinear source index along one axis (S -> D, float32): taps i0, i1 and weights l0, l1
+__device__ __forceinline__ void op_bilinear_tap(int S, int D, int d, int& i0, int& i1, float& l0, float& l1) {
+  const float scale = D > 1 ? __fdiv_rn((float)(S - 1), (float)(D - 1)) : 0.f;
+  const float src = __fmul_rn(scale, (float)d);
+  i0 = min((int)floorf(src), S - 1);
+  l1 = fminf(fmaxf(__fsub_rn(src, (float)i0), 0.f), 1.f);
+  l0 = __fsub_rn(1.f, l1);
+  i1 = i0 + (i0 < S - 1 ? 1 : 0);
+}
+
+// One CTA per (face, channel): F.interpolate(maps, (ch, cw), bilinear, align_corners=True) evaluated at every crop
+// pixel in float32, then the first maximum in raster order among the values > 0.05.  lmk int32 [F, 71, 2] = its crop
+// (x, y), or (-1, -1) when no value passes.
+__global__ void __launch_bounds__(256)
+op_face_peaks_kernel(const float* __restrict__ maps, int hs, int ws, const int* __restrict__ boxes,
+                     int* __restrict__ lmk) {
+  __shared__ float s_v[8];
+  __shared__ int s_i[8];
+  pdl_enter();
+  const int c = blockIdx.x, f = blockIdx.y, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int ch = boxes[f * 6 + 4], cw = boxes[f * 6 + 5];
+  const float* m = maps + ((long long)f * OP_FACE_MAPS + c) * hs * ws;
+  float best = -INFINITY;
+  int bi = -1;
+  for (int i = tid; i < ch * cw; i += blockDim.x) {
+    const int Y = i / cw, X = i % cw;
+    int y0, y1, x0, x1;
+    float a0, a1, b0, b1;
+    op_bilinear_tap(hs, ch, Y, y0, y1, a0, a1);
+    op_bilinear_tap(ws, cw, X, x0, x1, b0, b1);
+    const float t0 = __fadd_rn(__fmul_rn(m[y0 * ws + x0], b0), __fmul_rn(m[y0 * ws + x1], b1));
+    const float t1 = __fadd_rn(__fmul_rn(m[y1 * ws + x0], b0), __fmul_rn(m[y1 * ws + x1], b1));
+    const float v = __fadd_rn(__fmul_rn(t0, a0), __fmul_rn(t1, a1));
+    if (v > 0.05f && v > best) best = v, bi = i;          // i grows per thread: the first maximum is kept
+  }
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (oi >= 0 && (bi < 0 || ov > best || (ov == best && oi < bi))) best = ov, bi = oi;
+  }
+  if (lane == 0) s_v[warp] = best, s_i[warp] = bi;
+  __syncthreads();
+  if (tid == 0) {
+    for (int w = 1; w < 8; ++w)
+      if (s_i[w] >= 0 && (bi < 0 || s_v[w] > best || (s_v[w] == best && s_i[w] < bi))) best = s_v[w], bi = s_i[w];
+    int* o = lmk + ((long long)f * OP_FACE_MAPS + c) * 2;
+    o[0] = bi < 0 ? -1 : bi % cw;
+    o[1] = bi < 0 ? -1 : bi / cw;
+  }
+}
+
+// One warp per (face, landmark): Detector.detect_face's float32 normalisation ((p < 1e-6 ? -1 : p + x) / W), then
+// draw_facepose's int(x * W) (float32 products) and cv2.circle(r=3) where x > 0.01 and y > 0.01, drawn as slot
+// 35 + c of the face's person.
+__global__ void __launch_bounds__(OP_WARPS * 32)
+op_face_dots_kernel(const int* __restrict__ boxes, const int* __restrict__ lmk, int F, int H, int W,
+                    int* __restrict__ idx) {
+  pdl_enter();
+  const int lane = threadIdx.x & 31;
+  for (int d = blockIdx.x * OP_WARPS + threadIdx.x / 32; d < F * OP_FACE_MAPS; d += gridDim.x * OP_WARPS) {
+    const int f = d / OP_FACE_MAPS, c = d % OP_FACE_MAPS;
+    const int* b = boxes + f * 6;
+    const int lx = lmk[d * 2], ly = lmk[d * 2 + 1];
+    if (lx < 0) continue;                                 // the channel has no landmark
+    const float fx = __fdiv_rn(lx == 0 ? -1.f : (float)(lx + b[2]), (float)W);
+    const float fy = __fdiv_rn(ly == 0 ? -1.f : (float)(ly + b[3]), (float)H);
+    const int X = (int)__fmul_rn(fx, (float)W), Y = (int)__fmul_rn(fy, (float)H);
+    if (X > 0 && Y > 0)
+      op_circle<3>(idx + (long long)b[0] * H * W, H, W, X, Y, b[1] * OP_FACE_PRIMS + OP_PRIMS + c, lane);
   }
 }
 
@@ -846,11 +1050,81 @@ extern "C" PFD_API int pfd_openpose_draw_f32(const int32_t* persons, const int32
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (cudaMemsetAsync(idx, 0xff, sizeof(int32_t) * (size_t)B * H * W, st) != cudaSuccess)
     return set_error("pfd_openpose_draw_f32: memset failed");
-  launch_k(op_draw_kernel, dim3(OP_DRAW_BLOCKS, B), dim3(OP_WARPS * 32), (size_t)0, st,
+  launch_k(op_draw_kernel<OP_PRIMS>, dim3(OP_DRAW_BLOCKS, B), dim3(OP_WARPS * 32), (size_t)0, st,
            static_cast<const int*>(persons), static_cast<const int*>(npersons), static_cast<const int*>(xy), (int)H,
            (int)W, sintab, static_cast<int*>(idx));
   if (int rc = check_launch("openpose_draw")) return rc;
-  launch_k(op_color_kernel, dim3(grid_cap((long long)B * H * W, 256)), dim3(256), (size_t)0, st,
+  launch_k(op_color_kernel<OP_PRIMS>, dim3(grid_cap((long long)B * H * W, 256)), dim3(256), (size_t)0, st,
            static_cast<const int*>(idx), (int)B, (int)H, (int)W, static_cast<const unsigned char*>(colors), out);
   return check_launch("openpose_color");
+}
+
+extern "C" PFD_API int pfd_openpose_face_boxes(const int32_t* persons, const int32_t* npersons, const int32_t* xy,
+                                               int32_t B, int32_t H, int32_t W, int32_t* boxes, int32_t* count,
+                                               void* stream) {
+  if (!persons || !npersons || !xy || !boxes || !count || B <= 0 || H <= 0 || W <= 0)
+    return set_error("pfd_openpose_face_boxes: bad arguments (B=%d H=%d W=%d)", B, H, W);
+  launch_k(op_face_boxes_kernel, dim3(1), dim3(OP_BOX_THREADS), (size_t)0, static_cast<cudaStream_t>(stream),
+           static_cast<const int*>(persons), static_cast<const int*>(npersons), static_cast<const int*>(xy), (int)B,
+           (int)H, (int)W, static_cast<int*>(boxes), static_cast<int*>(count));
+  return check_launch("openpose_face_boxes");
+}
+
+extern "C" PFD_API int pfd_openpose_face_input_f16(const void* x, int32_t x_f32, int32_t B, int32_t H, int32_t W,
+                                                   int32_t n, int32_t cx, int32_t cy, int32_t ch, int32_t cw,
+                                                   int32_t D, int32_t mode, int32_t fy, int32_t fx, const int32_t* iy,
+                                                   const void* wy, int32_t ty, const int32_t* ix, const void* wx,
+                                                   int32_t tx, void* out, void* stream) {
+  if (!x || !out || B <= 0 || H <= 0 || W <= 0 || n < 0 || n >= B || cx < 0 || cy < 0 || ch <= 0 || cw <= 0 ||
+      cy + ch > H || cx + cw > W || D <= 0 || mode < 0 || mode > 4 || (mode == 0 && (ch != D || cw != D)) ||
+      (mode == 1 && (fy <= 0 || fx <= 0 || D * fy > ch || D * fx > cw)) ||
+      (mode >= 2 && (!axis_ok(iy, wy, ty) || !axis_ok(ix, wx, tx))) || (mode == 2 && (ty != 8 || tx != 8)) ||
+      (mode == 4 && (ty != 2 || tx != 2)))
+    return set_error("pfd_openpose_face_input_f16: bad arguments (B=%d %dx%d n=%d crop %d,%d %dx%d D=%d mode=%d)", B,
+                     H, W, n, cx, cy, ch, cw, D, mode);
+  if (misaligned(out)) return set_error("pfd_openpose_face_input_f16: out must be 16-byte aligned");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const OpAxis ay{iy, wy, ty}, ax{ix, wx, tx};
+  const int g = grid_cap((long long)D * D, 256);
+  if (x_f32)
+    launch_k(op_face_input_kernel<float>, dim3(g), dim3(256), (size_t)0, st, static_cast<const float*>(x), (int)H,
+             (int)W, (int)n, (int)cx, (int)cy, (int)D, (int)mode, (int)fy, (int)fx, ay, ax, static_cast<__half*>(out));
+  else
+    launch_k(op_face_input_kernel<__half>, dim3(g), dim3(256), (size_t)0, st, static_cast<const __half*>(x), (int)H,
+             (int)W, (int)n, (int)cx, (int)cy, (int)D, (int)mode, (int)fy, (int)fx, ay, ax, static_cast<__half*>(out));
+  return check_launch("openpose_face_input");
+}
+
+extern "C" PFD_API int pfd_openpose_face_peaks_f32(const float* maps, int32_t F, int32_t C, int32_t hs, int32_t ws,
+                                                   const int32_t* boxes, int32_t* lmk, void* stream) {
+  if (!maps || !boxes || !lmk || F <= 0 || F > 65535 || C != OP_FACE_MAPS || hs <= 0 || ws <= 0)
+    return set_error("pfd_openpose_face_peaks_f32: bad arguments (F=%d C=%d %dx%d)", F, C, hs, ws);
+  launch_k(op_face_peaks_kernel, dim3(OP_FACE_MAPS, F), dim3(256), (size_t)0, static_cast<cudaStream_t>(stream), maps,
+           (int)hs, (int)ws, static_cast<const int*>(boxes), static_cast<int*>(lmk));
+  return check_launch("openpose_face_peaks");
+}
+
+extern "C" PFD_API int pfd_openpose_face_draw_f32(const int32_t* persons, const int32_t* npersons, const int32_t* xy,
+                                                  int32_t B, int32_t H, int32_t W, const float* sintab,
+                                                  const uint8_t* colors, const int32_t* boxes, const int32_t* lmk,
+                                                  int32_t F, int32_t* idx, float* out, void* stream) {
+  if (!persons || !npersons || !xy || !sintab || !colors || !idx || !out || B <= 0 || B > 65535 || H <= 0 || W <= 0 ||
+      F < 0 || (F > 0 && (!boxes || !lmk)))
+    return set_error("pfd_openpose_face_draw_f32: bad arguments (B=%d H=%d W=%d F=%d)", B, H, W, F);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (cudaMemsetAsync(idx, 0xff, sizeof(int32_t) * (size_t)B * H * W, st) != cudaSuccess)
+    return set_error("pfd_openpose_face_draw_f32: memset failed");
+  launch_k(op_draw_kernel<OP_FACE_PRIMS>, dim3(OP_DRAW_BLOCKS, B), dim3(OP_WARPS * 32), (size_t)0, st,
+           static_cast<const int*>(persons), static_cast<const int*>(npersons), static_cast<const int*>(xy), (int)H,
+           (int)W, sintab, static_cast<int*>(idx));
+  if (int rc = check_launch("openpose_face_draw")) return rc;
+  if (F > 0) {
+    launch_k(op_face_dots_kernel, dim3(grid_cap((long long)F * OP_FACE_MAPS, OP_WARPS)), dim3(OP_WARPS * 32),
+             (size_t)0, st, static_cast<const int*>(boxes), static_cast<const int*>(lmk), (int)F, (int)H, (int)W,
+             static_cast<int*>(idx));
+    if (int rc = check_launch("openpose_face_dots")) return rc;
+  }
+  launch_k(op_color_kernel<OP_FACE_PRIMS>, dim3(grid_cap((long long)B * H * W, 256)), dim3(256), (size_t)0, st,
+           static_cast<const int*>(idx), (int)B, (int)H, (int)W, static_cast<const unsigned char*>(colors), out);
+  return check_launch("openpose_face_color");
 }

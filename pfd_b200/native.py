@@ -978,6 +978,56 @@ def openpose_draw(persons: torch.Tensor, npersons: torch.Tensor, xy: torch.Tenso
     return out
 
 
+def openpose_face_boxes(persons: torch.Tensor, npersons: torch.Tensor, xy: torch.Tensor, H: int, W: int):
+    """util.faceDetect of every person (pfd_openpose_face_boxes) -> (boxes int32 [B*MAX_PERSONS, 6] = (image, person,
+    x, y, ch, cw), compacted; count int32 [1])."""
+    B = persons.shape[0]
+    boxes = torch.empty((B * PFD_OPENPOSE_MAX_PERSONS, 6), device=persons.device, dtype=torch.int32)
+    count = torch.empty((1,), device=persons.device, dtype=torch.int32)
+    _call("pfd_openpose_face_boxes", persons, npersons, xy, B, H, W, boxes, count)
+    return boxes, count
+
+
+def openpose_face_input(x: torch.Tensor, n: int, box, D: int, plan, tabs, out: torch.Tensor) -> None:
+    """One face's network input into out (channel-last fp16 [D,D,16]): the crop box = (x, y, ch, cw) of image n,
+    cv2.resize to D x D by ``plan`` (openpose_tables.resize_plan, uint8), u8 / 256 - 0.5 (pfd_openpose_face_input_f16)."""
+    x, f32 = _chk_image(x, "openpose_face_input")
+    _chk16(out, "openpose_face_input out")
+    if tuple(out.shape) != (D, D, 16) or not out.is_contiguous():
+        raise RuntimeError(f"openpose_face_input: out must be a contiguous [{D},{D},16] tensor, got {tuple(out.shape)}")
+    B, _, H, W = x.shape
+    cx, cy, ch, cw = box
+    if plan[0] == "linear":
+        (iy, wy), (ix, wx) = tabs
+        mode, fy, fx, ay, ax = 4, 0, 0, (iy, wy, 2), (ix, wx, 2)
+    else:
+        mode, fy, fx, ay, ax = _plan_args(plan, tabs, u8=True)
+    _call("pfd_openpose_face_input_f16", x, f32, B, H, W, n, cx, cy, ch, cw, D, mode, fy, fx, *ay, *ax, out)
+
+
+def openpose_face_peaks(maps: torch.Tensor, boxes: torch.Tensor) -> torch.Tensor:
+    """maps fp32 [F,71,hs,ws], boxes int32 [>=F,6] -> landmarks int32 [F,71,2] in crop pixels, (-1, -1) where no value
+    of the align_corners bilinear map exceeds 0.05 (pfd_openpose_face_peaks_f32)."""
+    _chk32(maps, "openpose_face_peaks maps")
+    F, C, hs, ws = maps.shape
+    lmk = torch.empty((F, C, 2), device=maps.device, dtype=torch.int32)
+    _call("pfd_openpose_face_peaks_f32", maps, F, C, hs, ws, boxes, lmk)
+    return lmk
+
+
+def openpose_face_draw(persons: torch.Tensor, npersons: torch.Tensor, xy: torch.Tensor, H: int, W: int,
+                       sintab: torch.Tensor, colors: torch.Tensor, boxes: torch.Tensor, lmk: torch.Tensor,
+                       F: int) -> torch.Tensor:
+    """draw_poses with bodies and faces -> float32 [B,3,H,W] canvas / 255 (pfd_openpose_face_draw_f32); colors uint8
+    [106,3]."""
+    B = persons.shape[0]
+    dev = persons.device
+    idx = torch.empty((B, H, W), device=dev, dtype=torch.int32)
+    out = torch.empty((B, 3, H, W), device=dev, dtype=torch.float32)
+    _call("pfd_openpose_face_draw_f32", persons, npersons, xy, B, H, W, sintab, colors, boxes, lmk, F, idx, out)
+    return out
+
+
 def window_gather(x: torch.Tensor, ws: int, shift: int) -> torch.Tensor:
     B, H, W, C = x.shape
     Hp, Wp = -(-H // ws) * ws, -(-W // ws) * ws

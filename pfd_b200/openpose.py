@@ -209,27 +209,36 @@ class BodyPose(nn.Module):
         return store[key]
 
     @torch.no_grad()
-    def apply(self, x: torch.Tensor, debug: bool = False):
-        """x: CUDA [B,3,H,W] image in [0,1], fp16 or fp32 -> float32 [B,3,H,W] pose map (colour / 255), asynchronous on
-        the current stream.  debug=True also returns a dict of device tensors: 'maps' (fp32 [B,57,h',w'] stage-6 output,
-        PAFs then heatmaps), 'heatmaps' (fp32 [B,18,H,W]), 'peaks_xy' (int32 [B,18,MAX_PEAKS,2]), 'peaks_score'
-        (float64), 'peaks_total' (int32 [B,18], all peaks found), 'persons' (int32 [B,MAX_PERSONS,18], the peak index
-        within each part or -1), 'person_score' (float64 [B,MAX_PERSONS,2]: total score, parts) and 'npersons'."""
+    def detect(self, x: torch.Tensor, maps: Optional[torch.Tensor] = None):
+        """Body.__call__ for a CUDA [B,3,H,W] image in [0,1] without the drawing: the dict that apply(debug=True)
+        returns.  maps (fp32 [B,57,h',w'], PAFs then heatmaps) replaces the network's stage-6 output, so planted or
+        reference maps can be decoded."""
         if x.dim() != 4 or x.shape[1] != 3:
             raise ValueError(f"BodyPose.apply: expected a [B,3,H,W] image, got {tuple(x.shape)}")
         _, _, H, W = x.shape
         P = self._plans(H, W, x.device)
-        inp = nv.openpose_input(x, P["h"], P["w"], P["hp"], P["wp"], P["p_in"], P["t_in"])
-        maps = self.network(inp)
+        if maps is None:
+            maps = self.network(nv.openpose_input(x, P["h"], P["w"], P["hp"], P["wp"], P["p_in"], P["t_in"]))
         up = nv.openpose_resize(maps, 0, 57, P["h"], P["w"], P["p_up"], P["t_up"])
         heat = nv.openpose_resize(up, 38, 18, H, W, P["p_out"], P["t_out"])
         xy, score, total = nv.openpose_peaks(heat, P["gauss"])
         persons, pscore, npersons = nv.openpose_assemble(up, H, W, P["p_out"], P["t_out"], total, xy, score)
-        out = nv.openpose_draw(persons, npersons, xy, H, W, P["sintab"], P["colors"])
-        if not debug:
-            return out
-        return out, {"maps": maps, "heatmaps": heat, "peaks_xy": xy, "peaks_score": score, "peaks_total": total,
-                     "persons": persons, "person_score": pscore, "npersons": npersons}
+        return {"maps": maps, "heatmaps": heat, "peaks_xy": xy, "peaks_score": score, "peaks_total": total,
+                "persons": persons, "person_score": pscore, "npersons": npersons}
+
+    @torch.no_grad()
+    def apply(self, x: torch.Tensor, debug: bool = False, maps: Optional[torch.Tensor] = None):
+        """x: CUDA [B,3,H,W] image in [0,1], fp16 or fp32 -> float32 [B,3,H,W] pose map (colour / 255), asynchronous on
+        the current stream.  debug=True also returns a dict of device tensors: 'maps' (fp32 [B,57,h',w'] stage-6 output,
+        PAFs then heatmaps), 'heatmaps' (fp32 [B,18,H,W]), 'peaks_xy' (int32 [B,18,MAX_PEAKS,2]), 'peaks_score'
+        (float64), 'peaks_total' (int32 [B,18], all peaks found), 'persons' (int32 [B,MAX_PERSONS,18], the peak index
+        within each part or -1), 'person_score' (float64 [B,MAX_PERSONS,2]: total score, parts) and 'npersons'.
+        maps: given stage-6 maps instead of the network's (see detect)."""
+        info = self.detect(x, maps)
+        P = self._plans(x.shape[2], x.shape[3], x.device)
+        out = nv.openpose_draw(info["persons"], info["npersons"], info["peaks_xy"], x.shape[2], x.shape[3], P["sintab"],
+                               P["colors"])
+        return (out, info) if debug else out
 
 
 def _read_state_dict(path: str):

@@ -81,16 +81,41 @@ def area_axis(S: int, D: int):
     return idx, w
 
 
+def area_linear_axis(S: int, D: int):
+    """INTER_AREA along one axis when the other axis (or this one) enlarges: cv2.resize then emulates the area filter
+    with a bilinear variant (resize.cpp, area_mode of the generic path).  sx = floor(dx * S/D), fx = (dx + 1) -
+    (sx + 1) * D/S in float64, rounded to float32, 0 when <= 0 and else its fractional part; taps sx and
+    min(sx + 1, S - 1).  Weights are the uint8 path's int16 saturate_cast<short>((1 - fx) * 2048) and
+    saturate_cast<short>(fx * 2048) (an edge tap, sx = S - 1, always takes (2048, 0))."""
+    inv = D / S
+    scale = 1.0 / inv
+    idx = np.zeros((D, 2), np.int32)
+    w = np.zeros((D, 2), np.int32)
+    for d in range(D):
+        s = int(math.floor(d * scale))
+        f = np.float32((d + 1) - (s + 1) * inv)
+        f = np.float32(0) if f <= 0 else np.float32(f - np.float32(math.floor(f)))
+        if s >= S - 1:
+            s, f = S - 1, np.float32(0)
+        idx[d] = (s, min(s + 1, S - 1))
+        w[d] = (int(np.rint(np.float32(np.float32(1) - f) * np.float32(1 << COEF_BITS))),
+                int(np.rint(f * np.float32(1 << COEF_BITS))))
+    return idx, w
+
+
 def resize_plan(h: int, w: int, H: int, W: int, area: bool, fixed: bool):
     """How cv2.resize maps an h x w image to H x W with INTER_AREA (area=True) or INTER_LANCZOS4.
-    Returns ('copy',), ('block', fy, fx) for an integer-factor area reduction (resizeAreaFast), or
-    ('sep', (iy, wy), (ix, wx)) with separable tables."""
+    Returns ('copy',), ('block', fy, fx) for an integer-factor area reduction (resizeAreaFast),
+    ('sep', (iy, wy), (ix, wx)) with separable tables, or, for a uint8 INTER_AREA resize that enlarges along either
+    axis (fixed=True), ('linear', (iy, wy), (ix, wx)) with area_linear_axis tables."""
     if (h, w) == (H, W):
         return ("copy",)
     if area:
         sy, sx = 1.0 / (H / h), 1.0 / (W / w)
         if sy < 1 or sx < 1:
-            raise NotImplementedError(f"INTER_AREA enlargement {h}x{w} -> {H}x{W} is not used by the annotator")
+            if fixed:
+                return ("linear", area_linear_axis(h, H), area_linear_axis(w, W))
+            raise NotImplementedError(f"float INTER_AREA enlargement {h}x{w} -> {H}x{W} is not used by the annotator")
         iy, ix = int(round(sy)), int(round(sx))
         if abs(sy - iy) < np.finfo(np.float64).eps and abs(sx - ix) < np.finfo(np.float64).eps:
             return ("block", iy, ix)
